@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- the decoding hot path on N B200s: one JSON line with throughput, roofline, end-to-end and CPU-baseline
+"""bench.py -- the decoding hot path on N H100s: one JSON line with throughput, roofline, end-to-end and CPU-baseline
 figures for one workload.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl reference] [--no-extras]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W [--workload NAME]
 
@@ -20,6 +21,9 @@ their all-reduce (the only collective) is issued asynchronously once per step.  
 data-path collective (weak scaling, except turbo_c3 and link_c5 whose fixed totals -- 8,192 codewords, 1e8 symbols per
 point -- are split: strong).  `e2e` times the same
 work through the public host-buffer API (pinned host memory, H2D and D2H inside the timed region).
+`--dump-outputs DIR` writes what the last timed step computed as float32 / float64 .npy files (decoded bits: every frame,
+or a fixed seeded sample of frames when they exceed 32 MB); the inputs are seeded, so two builds can be compared output for
+output.
 `--impl reference` times the CPU restatement of the reference's algorithm (oracle/, fp64, all host threads) on the same
 workload -- the Python reference itself cannot travel to the GPU box (BASELINE.md section 2: ~1.5 codewords/s/core).
 """
@@ -36,7 +40,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-FALLBACK_HBM_GBS = 6650.0
+FALLBACK_HBM_GBS = 3350.0          # H100 SXM data sheet: 3.35 TB/s of HBM3
 HEADLINE_METRIC = "codewords/sec (K=7 rate-1/2 Viterbi, N=1024)"
 
 
@@ -71,17 +75,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json, burst copy bandwidth)"
         except Exception:
             pass
-    return FALLBACK_HBM_GBS, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(kernel):
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            return json.load(open(p)).get(kernel)
-        except Exception:
-            return None
-    return None
+    return FALLBACK_HBM_GBS, "H100 SXM data sheet (3.35 TB/s), not measured"
 
 
 def bind_to_gpu_numa_node(local_rank):
@@ -174,6 +168,21 @@ def count_errors(dec, msg, counters, torch):
     _lib.check(rc, "count_errors")
 
 
+DUMP_ARRAY_BYTES = 32 << 20          # per dumped array; a workload dumps one large array and a few small ones
+
+
+def sample_rows(t, seed=0):
+    """(rows, kept row indices) of a 2-D device tensor as float32: every row when it fits DUMP_ARRAY_BYTES, else a fixed,
+    seeded, sorted sample of rows"""
+    import torch
+    n = t.shape[0]
+    keep = max(1, DUMP_ARRAY_BYTES // (4 * t.shape[1]))
+    if n <= keep:
+        return t.float().cpu().numpy(), np.arange(n, dtype=np.float64)
+    idx = np.sort(np.random.RandomState(seed).choice(n, keep, replace=False))
+    return t[torch.from_numpy(idx).to(t.device)].float().cpu().numpy(), idx.astype(np.float64)
+
+
 # ------------------------------------------------------------------------------------------------ workloads
 class Workload:
     """One BASELINE config.  Subclasses fill in: describe() (IDENTICAL in both arms), make(), step(), units, roofline data,
@@ -203,16 +212,14 @@ class ViterbiWorkload(Workload):
         self.kernel = "viterbi_fast_kernel_%s<FFCode<6,0133,0171>>" % ("hard" if mode == "hard" else "soft")
         if metric:
             self.metric = metric
-        self.bound_note = ("add-compare-select issue bound, not HBM bound: 65,856 add-compare-selects per codeword; the "
-                           "kernel issues ~0.6 instructions per cycle and scheduler at ~239 instructions per trellis "
-                           "step and warp (DESIGN.md 4.1)")
+        self.bound_note = "add-compare-select issue bound, not HBM bound: 65,856 add-compare-selects per codeword"
 
     def describe(self):
         d = {"workload": self.name, "code": "K=7 (0o133,0o171) rate 1/2, 'cont'", "info_bits": self.nbits,
              "coded_values_per_frame": self.n_in, "decoding_type": self.mode, "tb_depth": 30,
              "frames_per_gpu": self.batch * self.launches, "frames_per_launch": self.batch,
              "alg_bytes_per_codeword": self.alg_bytes,
-             "l2": "every step streams %d distinct device batches (%.0f MB of input per step, > 126 MB L2)" % (
+             "l2": "every step streams %d distinct device batches (%.0f MB of input per step, > 50 MB L2)" % (
                  self.launches, self.launches * self.batch * self.n_in * (1 if self.mode == "hard" else 4) / 1e6)}
         d["channel"] = ("BSC p=%.3g" % self.flip) if self.mode == "hard" else ("BPSK AWGN Eb/N0=%.1f dB" % self.ebn0_db)
         return d
@@ -251,7 +258,9 @@ class ViterbiWorkload(Workload):
             self.inputs.append(x.contiguous())
             self.msgs.append(msg)
             del coded, pad
-        self.out = torch.empty((self.batch, self.nbits), dtype=torch.uint8, device="cuda")
+        # one output buffer per launch, so that the decisions of a whole step stay readable after it
+        self.outs = [torch.empty((self.batch, self.nbits), dtype=torch.uint8, device="cuda") for _ in range(self.launches)]
+        self.out = self.outs[0]
         self.kernel_launches_per_step = self.launches * (2 if self.mode == "hard" else 3)   # decode [+ frame scale] + count
 
     def step(self, torch, counters, ev=None):
@@ -259,10 +268,15 @@ class ViterbiWorkload(Workload):
         for i in range(self.launches):
             if ev is not None and i == 0:
                 ev[0].record()
-            viterbi_decode_batch(self.inputs[i], self.trellis, None, self.mode, out=self.out)
+            viterbi_decode_batch(self.inputs[i], self.trellis, None, self.mode, out=self.outs[i])
             if ev is not None and i == 0:
                 ev[1].record()
-            count_errors(self.out, self.msgs[i], counters, torch)
+            count_errors(self.outs[i], self.msgs[i], counters, torch)
+
+    def dump(self, torch):
+        """decoded bits of the last step: every launch's frames, in launch order"""
+        bits, rows = sample_rows(torch.cat(self.outs))
+        return {"decoded_bits": bits, "decoded_bits_rows": rows}
 
     def kernel_units(self):                      # units the event-timed launch processes
         return self.batch
@@ -371,7 +385,7 @@ class TurboWorkload(Workload):
                 "map_window": "commpy_b200.channelcoding.suggest_map_window(codewords per GPU, N): 1024 steps at 8,192 "
                               "codewords per GPU, 128 at 1,024 (CPB_OPT_BCJR_WINDOW; 96 warm-up steps either side always)",
                 "channel": "BPSK AWGN Eb/N0=1.0 dB, all-zero codewords", "alg_bytes_per_codeword": self.alg_bytes,
-                "l2": "inputs of one step (%.0f MB over all GPUs) exceed the 126 MB L2" % (3 * self.total * self.N * 4 / 1e6)}
+                "l2": "inputs of one step (%.0f MB over all GPUs) exceed the 50 MB L2" % (3 * self.total * self.N * 4 / 1e6)}
 
     def units_per_step(self, world):
         return self.total
@@ -398,10 +412,14 @@ class TurboWorkload(Workload):
         from commpy_b200.channelcoding import turbo_decode_batch
         if ev is not None:
             ev[0].record()
-        bits = turbo_decode_batch(self.y[0], self.y[1], self.y[2], self.trellis, self.s2, self.iters, self.il)
+        self.bits = turbo_decode_batch(self.y[0], self.y[1], self.y[2], self.trellis, self.s2, self.iters, self.il)
         if ev is not None:
             ev[1].record()
-        count_errors(bits, self.zero, counters, torch)
+        count_errors(self.bits, self.zero, counters, torch)
+
+    def dump(self, torch):
+        bits, rows = sample_rows(self.bits)
+        return {"decoded_bits": bits, "decoded_bits_rows": rows}
 
     def kernel_units(self):
         return self.batch
@@ -464,7 +482,7 @@ class LdpcWorkload(Workload):
         return {"workload": self.name, "code": "(64800, 32400) DVB-S2-SHAPED surrogate matrix (tests/helpers.py::dvbs2_like_H), 226,799 edges",
                 "algorithm": "MSA", "max_iterations": self.iters, "frames_per_gpu": self.batch,
                 "channel": "BPSK AWGN Eb/N0=1.0 dB, all-zero codeword", "alg_bytes_per_frame_iteration": 12 * 226799 + 8 * 64800,
-                "l2": "the messages of one step (%.0f MB) exceed the 126 MB L2" % (self.batch * 226799 * 4 / 1e6)}
+                "l2": "the messages of one step (%.0f MB) exceed the 50 MB L2" % (self.batch * 226799 * 4 / 1e6)}
 
     def units_per_step(self, world):
         return world * self.batch
@@ -492,8 +510,12 @@ class LdpcWorkload(Workload):
         dec, it = ldpc_bp_decode_batch(self.work, self.params, self.iters, "fp32", return_llrs=False, return_iters=True)
         if ev is not None:
             ev[1].record()
-        self.last_it = it
+        self.last_dec, self.last_it = dec, it
         count_errors(dec, self.zero, counters, torch)
+
+    def dump(self, torch):
+        bits, rows = sample_rows(self.last_dec)
+        return {"decoded_bits": bits, "decoded_bits_rows": rows, "iterations": self.last_it.double().cpu().numpy()}
 
     def kernel_units(self):
         return self.batch
@@ -589,6 +611,12 @@ class LinkWorkload(Workload):
         if ev is not None:
             ev[1].record()
         counters += tot
+        self.last_counters = tot
+
+    def dump(self, torch):
+        """BER per point and the summed [bit errors, frame errors, bits] of the last sweep"""
+        return {"ber_per_point": np.asarray(self.bers, dtype=np.float64),
+                "counters": self.last_counters.double().cpu().numpy()}
 
     def kernel_units(self):
         return self.units_per_step(1)
@@ -706,7 +734,7 @@ def run_reference(args):
     return 0
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ GPU arm
 def run_b200(args):
     import torch
     import torch.distributed as dist
@@ -765,6 +793,10 @@ def run_b200(args):
     e1.record()
     barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in wl.dump(torch).items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
     ms_total = e0.elapsed_time(e1)
     kernel_ms = float(np.mean([a.elapsed_time(b) for a, b in kev]))
     t = torch.tensor([ms_total, kernel_ms], dtype=torch.float64, device="cuda")
@@ -819,7 +851,7 @@ def run_b200(args):
         "parallelism": "frames sharded over %d GPU(s), no data-path collective; int64 error counters all-reduced "
                        "asynchronously once per step" % world,
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": ncu_traffic(wl.kernel), "kernel": wl.kernel, "kernel_ms": kernel_ms,
+                     "kernel": wl.kernel, "kernel_ms": kernel_ms,
                      "units_per_timed_launch": wl.kernel_units(), "peak_source": peak_src, "note": wl.bound_note},
         "gpu_launches": int(wl.kernel_launches_per_step * K),
         "clocks": clocks,
@@ -918,6 +950,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=DEFAULT_WORKLOAD, choices=sorted(WORKLOADS))
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (rank 0's frames) as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-"""commpy_b200 -- B200-native (sm_100a CUDA) implementation of CommPy's decoding hot path.
+"""commpy_b200 -- H100-native (sm_90a CUDA) implementation of CommPy's decoding hot path.
 
 Module layout mirrors the reference so that `import commpy_b200 as commpy` resolves the same names:
 

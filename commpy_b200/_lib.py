@@ -82,7 +82,7 @@ def release_scratch():
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise CommpyB200Error("commpy_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback.")
+        raise CommpyB200Error("commpy_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback.")
     return torch
 
 

@@ -1,9 +1,8 @@
-"""In-tree build of libcommpy_b200.so for sm_100a (nvcc cross-compiles without a GPU).
+"""In-tree build of libcommpy_b200.so for sm_90a (H100; nvcc cross-compiles without a GPU).
 
     python -m commpy_b200.build [--force] [--verbose]
 
-Objects go to build/, the shared library to commpy_b200/libcommpy_b200.so (git-ignored, but it travels
-to the GPU box with the gpurun snapshot)."""
+Objects go to build/, the shared library to commpy_b200/libcommpy_b200.so (both git-ignored)."""
 import os
 import subprocess
 import sys
@@ -16,9 +15,12 @@ OBJDIR = os.path.join(ROOT, "build")
 LIB = os.path.join(HERE, "libcommpy_b200.so")
 SOURCES = ["common.cu", "viterbi.cu", "bcjr.cu", "ldpc.cu", "demap.cu", "count.cu", "pipeline.cu", "hostapi.cu", "txlink.cu", "turbolink.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-         "-Xcompiler", "-fPIC", "--fmad=true",
-         "-DCPB_BUILDING=1"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
+                "-Xcompiler", "-fPIC", "--fmad=true",
+                "-DCPB_BUILDING=1"]
+# the compile command of the objects in build/: objects made with other flags (another architecture) are rebuilt
+STAMP = os.path.join(OBJDIR, "flags.txt")
 
 
 def _newer(target, deps):
@@ -30,6 +32,9 @@ def _newer(target, deps):
 
 def build(force=False, verbose=False):
     os.makedirs(OBJDIR, exist_ok=True)
+    cmdline = " ".join([NVCC] + FLAGS)
+    if not os.path.exists(STAMP) or open(STAMP).read() != cmdline:
+        force = True
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     headers.append(os.path.join(ROOT, "include", "commpy_b200.h"))
     srcs = [s for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
@@ -53,9 +58,10 @@ def build(force=False, verbose=False):
     with ThreadPoolExecutor(max(1, min(len(jobs), os.cpu_count() or 1))) as ex:
         list(ex.map(run, jobs))
     if force or jobs or _newer(LIB, objs):
-        cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
-                                                     "-Xcompiler", "-fPIC", "-lcudart"]
+        cmd = [NVCC, "-shared", "-o", LIB] + objs + ARCH + ["-Xcompiler", "-fPIC", "-lcudart"]
         run(cmd)
+    with open(STAMP, "w") as f:
+        f.write(cmdline)
     return LIB
 
 

@@ -115,7 +115,7 @@ def turbo_decode_batch_host(sys_symbols, non_sys_symbols_1, non_sys_symbols_2, t
 
 
 def suggest_map_window(batch, N, target_threads=49152):
-    """MAP window length (trellis steps per thread) that fills one B200 for `batch` frames of N steps: the kernels give every
+    """MAP window length (trellis steps per thread) that fills one GPU for `batch` frames of N steps: the kernels give every
     (frame, window) its own thread, so a small batch wants shorter windows (each pays 96 warm-up steps either side).
     Pass the result to `set_map_window`; the library default (1024) does not look at the batch, so that a frame decodes
     identically whatever it is batched with -- pinning ANY fixed window keeps that property."""

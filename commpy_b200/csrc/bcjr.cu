@@ -1,4 +1,4 @@
-// BCJR (MAP) decoding and the turbo loop on sm_100a -- replaces commpy/channelcoding/turbo.py:78-111
+// BCJR (MAP) decoding and the turbo loop on sm_90a -- replaces commpy/channelcoding/turbo.py:78-111
 // (_backward_recursion), :114-158 (_forward_recursion_decoding), :163-251 (map_decode) and the iteration
 // loop of :254-333 (turbo_decode).
 //
@@ -377,8 +377,8 @@ __global__ void __launch_bounds__(128) map_tpf_kernel(const Params p)
 // CK-th step.  The forward sweep then works segment by segment: reload the CK steps of inputs into shared memory,
 // recompute the segment's beta backwards from its checkpoint (same operations in the same order as the first
 // sweep, so the same values), then run alpha / the a-posteriori LLRs forwards.  This trades +1 beta recursion per
-// step for 8x less beta traffic: the plain kernel moved 4.7 GB per pass for a batch of 8192 x 6144 (3.2 GB of it
-// beta), i.e. it was HBM bound on non-algorithmic bytes (profiles/r01_other_kernels_ncu.md).
+// step for 8x less beta traffic: the plain kernel writes and reads beta for every step and state, 3.2 GB per pass for a
+// batch of 8192 x 6144 (8 states x 4 B each way), bytes the algorithm does not need to move.
 // Shared memory per thread: CK*(S+3) floats, thread-private columns [slot][thread] (conflict free).
 // ------------------------------------------------------------------------------------------------
 constexpr int CK = 8;
@@ -781,6 +781,7 @@ constexpr int PFF = CPB_MAP_PFF;
 #ifndef CPB_MAP_MINB
 #define CPB_MAP_MINB 12            // __launch_bounds__ minimum CTAs (= warps) per SM of map_lin2_kernel: <= 168 registers, three
                                    // warps per scheduler; the 1,536 warps of a config-3 pass (8,192 x 6 windows) are one wave
+                                   // on 132 SMs (1,584 slots)
 #endif
 template <class T, bool SM>      // SM: step-major arrays (Params::pitch / rmap)
 __global__ void __launch_bounds__(32, CPB_MAP_MINB) map_lin2_kernel(const Params p)
@@ -920,7 +921,7 @@ __global__ void __launch_bounds__(32, CPB_MAP_MINB) map_lin2_kernel(const Params
 #pragma unroll
         for (int i = 0; i < G; ++i) { vs[i] = q[i * bd]; vp[i] = q[(4 + i) * bd]; vl[i] = q[(8 + i) * bd]; }
         // (the interleaver entries of the group after next are requested BEFORE this group's copies: behind twelve DRAM
-        // misses in the load queue they came back too late -- 12 % of decoder 2's warp samples waited on them)
+        // misses in the load queue they come back too late)
         const int4 rcur = rnext;
         if (n + RB + 1 < ng) rnext = rows_of(first + (n + RB + 1) * stride);
         if (n + RB < ng) issue_group(ring_s + 4u * bd * 12 * slot, first + (n + RB) * stride, rcur);
@@ -953,7 +954,7 @@ __global__ void __launch_bounds__(32, CPB_MAP_MINB) map_lin2_kernel(const Params
         // The inputs of a group (4 steps) are fetched two groups ahead of their use into one of TWO statically named
         // register sets, the loop handles both per iteration.  (A rolled loop that rotates the sets by register moves makes
         // ptxas guard all of them with one scoreboard: the first use then waits for the loads issued half an iteration ago
-        // -- 26 % of all warp samples sat on that instruction.)
+        // -- the loads are exposed.)
         if constexpr (SM) {
             const int ng = (tb - lo) / G;
             stream_start(tb - G, -G, ng);
@@ -1267,7 +1268,7 @@ static int launch(const Params &p, bool vec, cudaStream_t st)
     unsigned grid = (unsigned)ceil_div(p.NT, 128);
     if (vec && (p.win % 4) == 0) {          // (a window that is not a multiple of CK ends in a 4-step segment)
         // one warp per CTA: 49,152 threads (C3: 8,192 frames x 6 windows) are 1,536 CTAs instead of 384, which
-        // spreads evenly over 148 SMs (measured 0.88 vs 0.91 ms per pass)
+        // spread more evenly over the SMs
         const int bd = 32;
         grid = (unsigned)ceil_div(p.NT, bd);
         const size_t smem = sizeof(float) * CK * (T::S + 3) * bd;
@@ -1332,7 +1333,7 @@ __global__ void __launch_bounds__(256) scatter_sub_kernel(const float *__restric
 
 // Row-staged forms of the three permutation kernels (one CTA per frame, the frame's row lives in shared memory):
 // the global side is fully coalesced and the random access of the interleaver happens in shared memory.
-// (The element-wise forms above issue one 32-byte sector request per 4-byte element: 0.35 ms per call at C3.)
+// (The element-wise forms above issue one 32-byte sector request per 4-byte element.)
 __global__ void __launch_bounds__(256) row_gather_sub_kernel(const float *__restrict__ a, const float *__restrict__ b,
                                                              const int32_t *__restrict__ perm, int N, float *__restrict__ out)
 {

@@ -64,9 +64,9 @@ int ensure_dyn_smem(const void *kernel, size_t bytes, bool max_carveout)
     auto it = done.find(key);
     if (it != done.end() && it->second >= bytes) return CPB_OK;
     CPB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    // kernels that get nothing from L1 ask for the largest shared-memory carve-out: the driver's own choice capped the
-    // step-major MAP kernel at 9 CTAs per SM where its registers allow 12.  (Not for kernels that re-read the other half
-    // of a 32-byte sector from L1, like the frame-major MAP kernel: measured 2x slower with the small L1.)
+    // kernels that get nothing from L1 ask for the largest shared-memory carve-out, so that the driver's own choice of
+    // carve-out cannot hold the step-major MAP kernel below the 12 CTAs per SM its registers allow.  (Not for kernels that
+    // re-read the other half of a 32-byte sector from L1, like the frame-major MAP kernel: they need the L1.)
     if (max_carveout)
         CPB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
     done[key] = bytes;
@@ -139,7 +139,7 @@ const char *cpb_strerror(int status)
     switch (status) {
     case CPB_OK: return "ok";
     case CPB_EINVAL: return "invalid argument";
-    case CPB_EUNSUPPORTED: return "configuration not supported by the B200 path";
+    case CPB_EUNSUPPORTED: return "configuration not supported by the H100 path";
     case CPB_ECUDA: return "CUDA runtime error (see cpb_last_cuda_error)";
     case CPB_ENOMEM: return "out of device memory";
     case CPB_ETRELLIS: return "trellis state without exactly 2^k predecessors";

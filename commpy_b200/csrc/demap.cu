@@ -1,4 +1,4 @@
-// PSK/QAM demapper on sm_100a -- replaces the triple loop of commpy/modulation.py:127-137
+// PSK/QAM demapper on sm_90a -- replaces the triple loop of commpy/modulation.py:127-137
 // (Modem.demodulate, 'soft') and the argmin of :121-123 ('hard').
 //
 //   LLR(bit b) = log sum_{k: bit b of k = 1} exp(-|y-c_k|^2/nv) - log sum_{k: bit b = 0} exp(-|y-c_k|^2/nv)

@@ -1,4 +1,4 @@
-// LDPC min-sum belief propagation on sm_100a -- replaces the per-edge Python loop of
+// LDPC min-sum belief propagation on sm_90a -- replaces the per-edge Python loop of
 // commpy/channelcoding/ldpc.py:229-238 (MSA check-node update), :243-248 (variable-node update) and the
 // early-stop test of :205, for a batch of blocks at once (the reference walks blocks sequentially, :197).
 //
@@ -176,8 +176,8 @@ __global__ void __launch_bounds__(256) cn_kernel(const int32_t *__restrict__ row
                     q[k].v[v] = x;
                     const T a = fabs(x);
                     neg[v] += (x < (T)0) ? 1 : 0;
-                    // (a branch-free fmin/fmax form was tried: fewer instructions, but ptxas then sinks the post loads next
-                    // to their uses and the pass gets slower -- 180 us vs 158 us at the DVB-S2 shape)
+                    // (a branch-free fmin/fmax form needs fewer instructions, but ptxas then sinks the post loads next
+                    // to their uses, which exposes their latency)
                     if (a < min1[v]) { min2[v] = min1[v]; min1[v] = a; arg[v] = k; }
                     else if (a < min2[v]) min2[v] = a;
                 }
@@ -248,8 +248,8 @@ __global__ void __launch_bounds__(256) cn_kernel(const int32_t *__restrict__ row
 // (check node i, frame chunk c): warp 0 asks the copy engine for the 2*deg rows of a tile (lane k <-> edge k) and an
 // mbarrier counts the bytes as they land; FT threads (one frame each) run the two-minimum update on the staged rows in
 // place; warp 0 hands the R rows back to the copy engine (bulk store).  NSTAGE tiles rotate, loads run NSTAGE-2 tiles
-// ahead, so the memory system always holds several KB per CTA in flight without a register being spent on it -- the
-// register-staged kernel above tops out at ~3.3 TB/s because its loads, math and stores share 16 warps per SM.
+// ahead, so the memory system always holds several KB per CTA in flight without a register being spent on it -- in the
+// register-staged kernel above, loads, math and stores share the same 16 warps per SM, which limits the bytes in flight.
 // Same arithmetic, same order: results are bit-identical to cn_kernel.
 namespace bulk {
 
@@ -649,7 +649,7 @@ static int run(const cpbLdpc *h, T *llr, int64_t batch, int n_iters, int spa, ui
                 { const int rc_ = ensure_dyn_smem(reinterpret_cast<const void *>(bulk::cn_bulk_kernel<T>), bulk_smem); if (rc_) { ws.release(); return rc_; } }
                 const DeviceProps &dp = device_props();
                 const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(4, (size_t)(220 * 1024) / (bulk_smem + 1024)));
-                int64_t want = (int64_t)(dp.sm_count > 0 ? dp.sm_count : 148) * per_sm;
+                int64_t want = (int64_t)(dp.sm_count > 0 ? dp.sm_count : 132) * per_sm;
                 want = std::max<int64_t>(nchunks, (want / nchunks) * nchunks);        // a multiple of nchunks
                 bulk_grid = (int)std::min<int64_t>((int64_t)h->m * nchunks, want);
             }

@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(128) conv_link_tx_kernel(const Params p)
 // ------------------------------------------------------------------------------------------------
 // Word-parallel form of the kernel above for the common link: n = 2 outputs per input bit, no puncturing, 2 / 4 / 8 bits per
 // symbol (QPSK, 16-QAM, 256-QAM) and frames of whole 128-bit message blocks.  Same random streams, same outputs (the test
-// suite compares the two kernels bit for bit), ~5x fewer instructions per symbol:
+// suite compares the two kernels bit for bit), far fewer instructions per symbol:
 //   * a thread owns ONE Philox message block (128 information bits = 256 / nb symbols) and encodes 32 bits at a time: the
 //     coded stream of output j is the XOR of the message word delayed by each set tap (funnel shifts across the word
 //     boundary) -- ~25 instructions per 32 bits instead of a popcount per bit and output;

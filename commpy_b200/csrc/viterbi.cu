@@ -1,4 +1,4 @@
-// Viterbi decoding on sm_100a -- replaces the loop nest of commpy/channelcoding/convcode.py:661-749
+// Viterbi decoding on sm_90a -- replaces the loop nest of commpy/channelcoding/convcode.py:661-749
 // (viterbi_decode), :590-657 (_acs_traceback), :575-587 (_compute_branch_metrics), :561-572 (_where_c).
 //
 // Exact semantics kept from the reference (SURVEY.md App. A.1):
@@ -104,10 +104,13 @@ constexpr int DMAX = 46;           // deepest traceback the fast path takes
 #endif
 constexpr int TASK_CAP = CPB_TASK_CAP;
 #ifndef CPB_VITERBI_TBB
-#define CPB_VITERBI_TBB 24         // windows per traceback block (multiple of B, <= 28)
+#define CPB_VITERBI_TBB 16         // windows per traceback block of the hard kernels (multiple of B, <= 28; a multiple of 8
+                                   // for packed output).  16 keeps the ring small enough for 8 CTAs per SM, so a 65,536-frame
+                                   // launch (1,024 CTAs) is one wave on 132 SMs; 24 fits 7 (profiles/h100_viterbi_tbb.md)
 #endif
 #ifndef CPB_VITERBI_TBB_SOFT
-#define CPB_VITERBI_TBB_SOFT CPB_VITERBI_TBB    // the same for the one-frame-per-thread (float input) kernels
+#define CPB_VITERBI_TBB_SOFT 24    // the same for the one-frame-per-thread (float input) kernels: their CTAs per SM are set by
+                                   // registers, not by the ring, so a smaller block would not add a CTA
 #endif      // retired paths kept per block and warp; beyond that they are finished inline
 
 struct Params {
@@ -443,7 +446,8 @@ __device__ __noinline__ void tb_block_call(const Smem<PACK> sm, int ts, int te, 
 #define CPB_QD_SOFT 2              // input prefetch distance of the soft kernels, in pairs of steps
 #endif
 #ifndef CPB_SOFT_MIN_CTAS
-#define CPB_SOFT_MIN_CTAS 8        // __launch_bounds__ minimum CTAs per SM of the soft kernels (12 -- a 168-register cap -- measured 2.7 % slower)
+#define CPB_SOFT_MIN_CTAS 8        // __launch_bounds__ minimum CTAs per SM of the soft kernels (a 255-register cap; on sm_90a the
+                                   // K=7 kernels need 156, under the 168 of 12 CTAs as well)
 #endif
 #ifndef CPB_TB_DEPHASE
 #define CPB_TB_DEPHASE 8           // windows in the first traceback block of the second warp of a scheduler (0: off)
@@ -697,8 +701,8 @@ __device__ __forceinline__ void viterbi_fast_body(const Params &p)
     uint32_t mq0 = 0u, mq1 = 0u;                 // best fields of the first half of the running block
     static_assert(QD >= 2 && QD % 2 == 0, "the prefetch queue moves by whole blocks");
     const int npairs = p.T >> 1, nfull = p.T >> 2;
-    // (A loop body of half a block -- smaller code -- was measured: slower, the register shuffling at the extra loop
-    // edge costs more than the instruction fetch it saves.)
+    // (A loop body of half a block -- smaller code -- adds register shuffling at the extra loop edge in exchange for the
+    // instruction fetch it saves.)
 #pragma unroll 1
     for (int blk = 0; blk < nfull; ++blk) {
         const Raw cur0 = gather(qd[0]), cur1 = gather(qd[1]);

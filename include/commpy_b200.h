@@ -1,5 +1,5 @@
 /*
- * commpy_b200.h -- C-ABI of libcommpy_b200.so: CommPy's decoding hot path on B200 (sm_100a).
+ * commpy_b200.h -- C-ABI of libcommpy_b200.so: CommPy's decoding hot path on H100 (sm_90a).
  *
  * The reference (veeresht/CommPy @ 9aecd7c) has no FFI layer: the hot path sits behind plain
  * Python functions.  Each entry point below names the reference function whose loop nest it
@@ -70,7 +70,7 @@ typedef struct cpbTrellis cpbTrellis;
 int cpb_trellis_create(const int32_t *next_state_host, const int32_t *output_host,
                        int k, int n, int total_memory, int number_states, cpbTrellis **out);
 int cpb_trellis_destroy(cpbTrellis *t);
-/* 0 = generic table-driven kernels; >0 = id of the register-resident sm_100a fast path that matched. */
+/* 0 = generic table-driven kernels; >0 = id of the register-resident fast path that matched. */
 int cpb_trellis_fast_path(const cpbTrellis *t);
 
 /* ---- Viterbi: convcode.py:661-749 viterbi_decode (+ :590-657 _acs_traceback, :575-587 metrics) - */

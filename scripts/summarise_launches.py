@@ -1,4 +1,4 @@
-"""Turn an `ncu --metrics gpu__time_duration.sum --csv` launch list into the markdown table kept under profiles/."""
+"""Turn an `ncu --metrics gpu__time_duration.sum --csv` launch list into a markdown table."""
 import csv
 import sys
 from collections import OrderedDict

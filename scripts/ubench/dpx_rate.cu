@@ -1,4 +1,4 @@
-// Micro-benchmark: issue rate and latency of the integer min/add-min instructions the Viterbi kernels use (sm_100a).
+// Micro-benchmark: issue rate and latency of the integer min/add-min instructions the Viterbi kernels use (sm_90a).
 // One warp per CTA, one CTA per SM sub-partition is enough: cycles per warp instruction = rt of the pipe.
 #include <cstdio>
 #include <cstdint>

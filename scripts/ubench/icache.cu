@@ -1,6 +1,7 @@
 // Micro-benchmark: does a long straight-line loop body (like the unrolled add-compare-select block) run at full issue
 // rate, or does instruction fetch limit it?  Body = N pairs (VIADDMNMX + IMAD) over 16 independent chains.
 #include <cstdio>
+#include <vector>
 #include <cstdint>
 #include <cuda_runtime.h>
 
@@ -26,15 +27,15 @@ __global__ void k(uint32_t *out, long long *cyc, uint32_t seed, int iters)
 }
 
 template <int NPAIR>
-void run(uint32_t *out, long long *cyc)
+void run(uint32_t *out, long long *cyc, int nsm)
 {
     for (int warps : {1, 4, 8}) {
         const int iters = 65536 / NPAIR;
-        k<NPAIR><<<148, 32 * warps>>>(out, cyc, 12345, iters);
-        long long h[148];
-        cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
-        double m = 0; for (int i = 0; i < 148; ++i) m += (double)h[i];
-        m /= 148;
+        k<NPAIR><<<nsm, 32 * warps>>>(out, cyc, 12345, iters);          // one CTA per SM
+        std::vector<long long> h(nsm);
+        cudaMemcpy(h.data(), cyc, sizeof(long long) * nsm, cudaMemcpyDeviceToHost);
+        double m = 0; for (int i = 0; i < nsm; ++i) m += (double)h[i];
+        m /= nsm;
         printf("body %5d instr (%6.1f KB): warps/SM %d: %.3f cycles per instruction per warp, %.3f IPC per SMSP\n", 2 * NPAIR, 2 * NPAIR * 16 / 1024.0,
                warps, m / ((double)iters * 2 * NPAIR), (warps >= 4 ? warps / 4.0 : 1.0) * (double)iters * 2 * NPAIR / m);
     }
@@ -43,8 +44,10 @@ void run(uint32_t *out, long long *cyc)
 int main()
 {
     uint32_t *out; long long *cyc;
-    cudaMalloc(&out, 1 << 22); cudaMalloc(&cyc, 8 * 148);
-    run<64>(out, cyc); run<128>(out, cyc); run<256>(out, cyc); run<384>(out, cyc); run<512>(out, cyc); run<768>(out, cyc);
-    run<1024>(out, cyc); run<2048>(out, cyc); run<4096>(out, cyc);
+    int nsm = 0;
+    cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, 0);
+    cudaMalloc(&out, 1 << 22); cudaMalloc(&cyc, sizeof(long long) * nsm);
+    run<64>(out, cyc, nsm); run<128>(out, cyc, nsm); run<256>(out, cyc, nsm); run<384>(out, cyc, nsm); run<512>(out, cyc, nsm);
+    run<768>(out, cyc, nsm); run<1024>(out, cyc, nsm); run<2048>(out, cyc, nsm); run<4096>(out, cyc, nsm);
     return 0;
 }

@@ -1,5 +1,5 @@
 """CPU: the oracle (oracle/commpy_oracle.c) against the golden vectors generated from the UNMODIFIED reference
-by oracle/validate_against_reference.py.  This is what pins the oracle on machines without /root/reference."""
+by oracle/validate_against_reference.py.  This is what pins the oracle without the reference checkout."""
 import os
 
 import numpy as np

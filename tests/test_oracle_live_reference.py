@@ -1,130 +1,99 @@
-"""Live pin of the oracle: where the reference checkout is present (the build container; never the GPU box), fresh random
-cases -- not the committed goldens -- are run through the UNMODIFIED reference and through oracle/commpy_oracle.c and must
-agree (bit-exact for Viterbi and LDPC min-sum incl. out_llrs, 1e-9 for the float outputs).  Skipped elsewhere."""
+"""CPU: the oracle (oracle/commpy_oracle.c) and the host-side MIMO mirrors against outputs of the UNMODIFIED reference on
+cases drawn from several fixed seeds (tests/golden/live_reference.npz, written by oracle/make_live_golden.py): bit-exact for
+Viterbi, LDPC min-sum incl. out_llrs and the hard demapper, 1e-9 for the float outputs."""
 import os
-import time
-import warnings
 
 import numpy as np
 import pytest
+import scipy.sparse as sp
 
-from oracle import oracle, refimport
+import helpers
+from oracle import oracle
 
-pytestmark = [pytest.mark.skipif(not refimport.available(), reason="reference checkout not present"),
-              pytest.mark.filterwarnings("ignore")]
+pytestmark = pytest.mark.filterwarnings("ignore")
 
-
-@pytest.fixture(scope="module")
-def ref():
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        refimport.import_reference()
-        import commpy.channelcoding as rcc
-        import commpy.modulation as rmod
-    return rcc, rmod
+GOLD = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live_reference.npz"))
+TAGS = ["s%d" % s for s in GOLD["seeds"]]
 
 
-def _seed():
-    return int(time.time()) % (1 << 31)          # a different draw every run; printed on failure
+def test_viterbi_and_bcjr_fresh_cases():
+    """Viterbi (every mode and termination) and BCJR with a prior on the stored cases of every seed.  ("fresh": cases other
+    than those of tests/golden/viterbi.npz and bcjr_turbo.npz; they come from fixed seeds, not from each run.)"""
+    for tag in TAGS:
+        _viterbi_and_bcjr(GOLD, tag)
 
 
-def test_viterbi_and_bcjr_fresh_cases(ref):
-    rcc, _ = ref
-    seed = _seed()
-    rs = np.random.RandomState(seed)
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        k7 = rcc.Trellis(np.array([6]), np.array([[0o133, 0o171]]))
-        rsc = rcc.Trellis(np.array([3]), np.array([[1, 0o15]]), np.array([[0o13]]), "rsc")
+def _viterbi_and_bcjr(g, tag):
+    k7 = helpers.k7()
     for mode in ("hard", "soft", "unquantized"):
-        for term, tb in (("cont", None), ("term", 9)):
-            msg = rs.randint(0, 2, 48)
-            c = rcc.conv_encode(msg, k7, term).astype(float)
-            if mode == "hard":
-                x = np.abs(c - (rs.rand(len(c)) < 0.1))
-            elif mode == "soft":
-                x = (2 * c - 1) * 2 + rs.randn(len(c)) * 2.5
-            else:
-                x = (2 * c - 1) + rs.randn(len(c))
-            want = rcc.viterbi_decode(x.copy(), k7, tb, mode)
-            assert np.array_equal(want, oracle.viterbi_decode(x.copy(), k7, tb, mode)), (seed, mode, term, tb)
-    N = 40
-    s2 = 0.9
-    sys_, par, la = (-1 + np.sqrt(s2) * rs.randn(N) for _ in range(3))
-    with np.errstate(all="ignore"):
-        want = rcc.map_decode(sys_, par, rsc, s2, 0.2 * la, "decode")
-    got = oracle.map_decode(sys_, par, rsc, s2, 0.2 * la, "decode")
-    assert np.allclose(want[0], got[0], rtol=1e-9, atol=1e-9) and np.array_equal(want[1], got[1]), seed
+        for term in ("cont", "term"):
+            key = "%s_vit_%s_%s" % (tag, mode, term)
+            tb = int(g[key + "_tb"]) or None
+            assert np.array_equal(g[key + "_ref"], oracle.viterbi_decode(g[key + "_x"].copy(), k7, tb, mode)), key
+    got = oracle.map_decode(g[tag + "_map_sys"], g[tag + "_map_par"], helpers.rsc_k4(), float(g[tag + "_map_s2"]),
+                            g[tag + "_map_La"], "decode")
+    assert np.allclose(g[tag + "_map_L"], got[0], rtol=1e-9, atol=1e-9) and np.array_equal(g[tag + "_map_bits"], got[1]), tag
 
 
-def test_ldpc_and_demapper_fresh_cases(ref):
-    rcc, rmod = ref
-    seed = _seed() + 1
-    rs = np.random.RandomState(seed)
-    design = os.path.join(refimport.REF_ROOT, "commpy/channelcoding/designs/ldpc/gallager/96.33.964.txt")
-    params = rcc.get_ldpc_code_params(design)
-    sigma = 0.9
-    llr = 2.0 * (1.0 + sigma * rs.randn(2 * 96)) / sigma ** 2
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        want_dec, want_out = rcc.ldpc_bp_decode(llr.copy(), params, "MSA", 6)
-    dec, out = oracle.ldpc_bp_decode(llr.copy(), params, "MSA", 6)
-    assert np.array_equal(want_dec, dec) and np.array_equal(want_out, out), seed
-    modem = rmod.QAMModem(16)
-    y = modem.modulate(rs.randint(0, 2, 4 * 30)) + 0.4 * (rs.randn(30) + 1j * rs.randn(30))
-    with np.errstate(all="ignore"):
-        want = modem.demodulate(y, "soft", 0.7)
+def test_ldpc_and_demapper_fresh_cases():
+    """LDPC min-sum on the gallager 96.33.964 design and the 16-QAM demapper on the stored cases of every seed (fixed seeds)"""
+    for tag in TAGS:
+        _ldpc_and_demapper(GOLD, tag)
+
+
+def _ldpc_and_demapper(g, tag):
+    from commpy_b200.modulation import QAMModem
+    m, n = (int(v) for v in g["ldpc_H_shape"])
+    H = sp.csr_matrix((np.ones(len(g["ldpc_H_indices"]), np.int8), g["ldpc_H_indices"], g["ldpc_H_indptr"]), shape=(m, n))
+    params = {"n_vnodes": n, "parity_check_matrix": H}
+    dec, out = oracle.ldpc_bp_decode(g[tag + "_ldpc_llr"].copy(), params, "MSA", 6)
+    assert np.array_equal(g[tag + "_ldpc_dec"], dec) and np.array_equal(g[tag + "_ldpc_out"], out), tag
+    modem = QAMModem(16)
+    y = g[tag + "_demap_y"]
+    want = g[tag + "_demap_soft"]
     got = oracle.demodulate(modem, y, "soft", 0.7)
     fin = np.isfinite(want)
-    assert np.allclose(want[fin], got[fin], rtol=1e-9, atol=1e-9), seed
-    assert np.array_equal(modem.demodulate(y, "hard"), oracle.demodulate(modem, y, "hard")), seed
+    assert np.allclose(want[fin], got[fin], rtol=1e-9, atol=1e-9), tag
+    assert np.array_equal(g[tag + "_demap_hard"], oracle.demodulate(modem, y, "hard")), tag
 
 
-def test_mimo_mirrors_fresh_cases(ref):
-    """host-side MIMO mirrors (kbest, best_first_detector, idd_decoder) against the live reference on fresh draws"""
-    import importlib
-    _, rmod = ref
-    rlinks = importlib.import_module("commpy.links")
+def test_mimo_mirrors_fresh_cases():
+    """host-side MIMO mirrors (kbest, best_first_detector, idd_decoder) against the reference's outputs on the stored cases
+    of every seed (fixed seeds)"""
+    for tag in TAGS:
+        _mimo_mirrors(GOLD, tag)
+
+
+def _mimo_mirrors(g, tag):
     from commpy_b200 import modulation as mod
     from commpy_b200.links import idd_decoder
-    seed = _seed()
-    rs = np.random.RandomState(seed)
     for m, n in ((4, 2), (16, 3), (16, 4)):
-        rq = rmod.QAMModem(m)
         mq = mod.QAMModem(m)
-        np.testing.assert_array_equal(rq.constellation, mq.constellation)
 
         def demode(s):
-            return rq.demodulate(s, "hard")
-        for _ in range(10):
-            nb = rq.num_bits_symbol
-            h = (rs.randn(n, n) + 1j * rs.randn(n, n)) * np.sqrt(0.5)
-            nv = n / 10 ** (rs.uniform(5, 25) / 10)
-            y = h.dot(rq.modulate(rs.randint(0, 2, n * nb))) + (rs.randn(n) + 1j * rs.randn(n)) * np.sqrt(nv / 2)
-            msg = "seed %d" % seed
-            np.testing.assert_allclose(mod.kbest(y, h, mq.constellation, 6), rmod.kbest(y, h, rq.constellation, 6), atol=1e-12,
-                                       err_msg=msg)
-            np.testing.assert_allclose(mod.kbest(y, h, mq.constellation, 6, nv, "soft", demode),
-                                       rmod.kbest(y, h, rq.constellation, 6, nv, "soft", demode), rtol=1e-9, atol=1e-9, err_msg=msg)
-            stack = tuple(rs.randint(1, 6, n - 1))
+            return oracle.demodulate(mq, s, "hard")
+        key = "%s_mimo_q%d_n%d" % (tag, m, n)
+        for c in range(len(g[key + "_y"])):
+            y, h, nv = g[key + "_y"][c], g[key + "_h"][c], float(g[key + "_nv"][c])
+            stack = tuple(int(s) for s in g[key + "_stack"][c])
+            msg = "%s case %d" % (key, c)
+            np.testing.assert_allclose(mod.kbest(y, h, mq.constellation, 6), g[key + "_kbest_hard"][c], atol=1e-12, err_msg=msg)
+            np.testing.assert_allclose(mod.kbest(y, h, mq.constellation, 6, nv, "soft", demode), g[key + "_kbest_soft"][c],
+                                       rtol=1e-9, atol=1e-9, err_msg=msg)
             np.testing.assert_allclose(mod.best_first_detector(y, h, mq.constellation, stack, nv, demode, 100),
-                                       rmod.best_first_detector(y, h, rq.constellation, stack, nv, demode, 100), rtol=1e-9,
-                                       atol=1e-9, err_msg=msg)
-    # idd_decoder: same closures through both, 3 iterations
-    rq = rmod.QAMModem(16)
+                                       g[key + "_best_first"][c], rtol=1e-9, atol=1e-9, err_msg=msg)
+    # idd_decoder: the reference's closures, with the mirrors' kbest, 3 iterations
+    mq = mod.QAMModem(16)
 
     def detector(y, h, constellation, noise_var, a_priori):
-        return rmod.kbest(y, h, constellation, 8, noise_var, "soft", lambda s: rq.demodulate(s, "hard")) + 0.25 * a_priori
+        return mod.kbest(y, h, constellation, 8, noise_var, "soft", lambda s: oracle.demodulate(mq, s, "hard")) + 0.25 * a_priori
 
     def decoder(llr):
         return np.tanh(llr) * 3 + np.roll(llr, 1)
 
     def decision(llr):
         return (llr > 0).astype(int)
-    nvec, n = 5, 2
-    h = (rs.randn(nvec, n, n) + 1j * rs.randn(nvec, n, n)) * np.sqrt(0.5)
-    y = np.einsum("ijk,ik->ij", h, rq.modulate(rs.randint(0, 2, nvec * n * 4)).reshape(nvec, n)) + 0.1 * rs.randn(nvec, n)
-    ap = rs.randn(nvec * n * 4)
-    got = idd_decoder(detector, decoder, decision, 3)(y, h, rq.constellation, 0.02, ap.copy(), n * 4)
-    want = rlinks.idd_decoder(detector, decoder, decision, 3)(y, h, rq.constellation, 0.02, ap.copy(), n * 4)
-    np.testing.assert_array_equal(got, want)
+    n = 2
+    got = idd_decoder(detector, decoder, decision, 3)(g[tag + "_idd_y"], g[tag + "_idd_h"], mq.constellation, 0.02,
+                                                     g[tag + "_idd_ap"].copy(), n * 4)
+    np.testing.assert_array_equal(got, g[tag + "_idd_ref"])
