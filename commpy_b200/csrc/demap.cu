@@ -287,6 +287,7 @@ int cpb_demod_soft(const cpbModem *m, const float *y_dev, int64_t n_sym, float n
         case 3: demap::demod_soft_separable<3><<<grid, 256, 0, st>>>(y, n_sym, tab, inv, llr_dev); break;
         case 4: demap::demod_soft_separable<4><<<grid, 256, 0, st>>>(y, n_sym, tab, inv, llr_dev); break;
         case 5: demap::demod_soft_separable<5><<<grid, 256, 0, st>>>(y, n_sym, tab, inv, llr_dev); break;
+        case 6: demap::demod_soft_separable<6><<<grid, 256, 0, st>>>(y, n_sym, tab, inv, llr_dev); break;
         default: return CPB_EUNSUPPORTED;
         }
         CPB_LAUNCH_CHECK();

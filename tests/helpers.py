@@ -15,6 +15,16 @@ def k7_wifi_quirk():
     return Trellis(np.array([6]), np.array([[133, 171]]))
 
 
+def k7_171_133():
+    """The K=7 code with its two generators swapped (octal 171, 133)."""
+    return Trellis(np.array([6]), np.array([[0o171, 0o133]]))
+
+
+def mem6_5_7():
+    """Trellis([6], [[5, 7]]): the 64-state trellis of commpy/channelcoding/README.md:81-84."""
+    return Trellis(np.array([6]), np.array([[5, 7]]))
+
+
 def reference_test_trellises():
     """The five trellises of commpy/channelcoding/tests/test_convcode.py:23-111."""
     with warnings.catch_warnings():
@@ -109,6 +119,50 @@ def dvbs2_like_H(seed=3, n=64800, m=32400, n8=12960, n3=19440):
     H.data[:] = 1
     H.sort_indices()
     return H
+
+
+def mixed_degree_H(row_degrees, n, seed=0):
+    """Parity-check matrix with the given row degrees (one row per entry) over n columns, edges placed at random without
+    repeats; every column gets at least one edge when the degrees allow it.  Returns a scipy CSR int8 matrix."""
+    import scipy.sparse as sp
+    rs = np.random.RandomState(seed)
+    rows, cols = [], []
+    unused = list(rs.permutation(n))
+    for i, d in enumerate(row_degrees):
+        take = [unused.pop() for _ in range(min(d, len(unused)))]
+        rest = np.setdiff1d(np.arange(n), take)
+        take += list(rs.choice(rest, d - len(take), replace=False))
+        rows += [i] * d
+        cols += take
+    H = sp.csr_matrix((np.ones(len(rows), np.int8), (rows, cols)), shape=(len(row_degrees), n))
+    H.sort_indices()
+    return H
+
+
+def normalize_kernel_name(name):
+    """Kernel name without spaces, integer casts and integer suffixes, so that the profiler's demangling
+    ('FFCode<6, 5u, 7u>') and cu++filt's ('FFCode<(int)6, (unsigned int)5, (unsigned int)7>') compare equal."""
+    import re
+    s = re.sub(r"\((?:unsigned |signed )?(?:int|long long|long|short|char)\)", "", name)
+    s = s.replace(" ", "")
+    return re.sub(r"(?<=\d)(?:ull|ll|ul|u|l)(?=[,>)])", "", s)
+
+
+def launched_kernels(fn):
+    """Run fn() under torch.profiler (CUDA activity only: CUPTI sees every kernel of the process, including the ones the
+    ctypes library launches on its own pipeline streams) and return the normalised names of what it recorded: the
+    kernels launched, plus the runtime API calls (cudaLaunchKernel, ...) that made them."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    names = {e.name for e in prof.events()}
+    raw = getattr(prof.profiler, "kineto_results", None)                     # the raw activity records, when exposed
+    if raw is not None:
+        names |= {e.name() for e in raw.events()}
+    return {normalize_kernel_name(s) for s in names if not s.startswith(("Memcpy", "Memset"))}
 
 
 # ---- NumPy model of the device-side TX chain (commpy_b200/csrc/txlink.cu) ------------------------------------------

@@ -13,7 +13,7 @@ def _agree(got, want):
     return float((np.asarray(got) == np.asarray(want)).mean())
 
 
-@pytest.mark.parametrize("make", [helpers.k7, helpers.k7_wifi_quirk])
+@pytest.mark.parametrize("make", [helpers.k7, helpers.k7_wifi_quirk, helpers.k7_171_133, helpers.mem6_5_7])
 @pytest.mark.parametrize("tb", [None, 15, 7, 46, 48])
 @pytest.mark.parametrize("term", ["cont", "term"])
 def test_k7_hard_bit_exact(make, tb, term):
