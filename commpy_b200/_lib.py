@@ -26,7 +26,8 @@ SYMBOLS = [
     "cpb_map_decode_host", "cpb_turbo_decode_host", "cpb_ldpc_decode_host", "cpb_demod_soft_host",
     "cpb_ldpc_create", "cpb_ldpc_destroy", "cpb_ldpc_workspace_bytes", "cpb_ldpc_minsum", "cpb_ldpc_sumproduct",
     "cpb_modem_create", "cpb_modem_destroy", "cpb_modem_is_separable", "cpb_demod_soft", "cpb_demod_hard",
-    "cpb_count_errors", "cpb_conv_link_tx", "cpb_conv_link_tx_punctured", "cpb_turbo_link_tx",
+    "cpb_demod_soft_csi", "cpb_demod_hard_csi",
+    "cpb_count_errors", "cpb_conv_link_tx", "cpb_conv_link_tx_punctured", "cpb_conv_link_tx_fading", "cpb_turbo_link_tx",
 ]
 
 _lib = None

@@ -13,6 +13,10 @@
 // Philox(counter = (f_lo, f_hi, q, 1), key = seed) through Box-Muller.  Results therefore do not depend on the launch
 // geometry, the batch split or the number of GPUs (each rank passes its own first_frame), SURVEY 8(e).
 //
+// Flat fading (FADING = true, cpb_conv_link_tx_fading; SISOFlatChannel, commpy/channels.py:176-221): the gains of symbols
+// 2q, 2q+1 of frame f come from Philox(counter = (f_lo, f_hi, q, 5), key = seed) through the same Box-Muller,
+// h = los + nlos_std (g.x + j g.y), and y = h c + sigma n with the noise n above; h is written out next to y.
+//
 // Encoder: k = 1 feed-forward shift register; tap mask g_j bit b multiplies the input delayed by b (bit 0 = current
 // input) -- derived on the host from the Trellis tables and verified against every (state, input) entry.
 #include <cmath>
@@ -45,6 +49,9 @@ struct Params {
     const float2 *cst;
     uint8_t *msg;
     float2 *y;
+    float los_re, los_im;     // fading: mean gain and per-component std of its scattered part
+    float nlos_std;
+    float2 *h;                // fading gains, same layout as y
 };
 
 __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1)
@@ -70,6 +77,19 @@ __device__ __forceinline__ float2 box_muller(uint32_t a, uint32_t b)
     return make_float2(r * cs, r * sn);
 }
 
+// fading gain of one symbol from two standard normals
+__device__ __forceinline__ float2 fading_gain(const Params &p, float2 g)
+{
+    return make_float2(fmaf(p.nlos_std, g.x, p.los_re), fmaf(p.nlos_std, g.y, p.los_im));
+}
+
+// h * c; exact at h = 1 + 0j (1 * c.x - 0 * c.y is c.x whichever product the compiler fuses)
+__device__ __forceinline__ float2 cmul(float2 h, float2 c)
+{
+    return make_float2(h.x * c.x - h.y * c.y, h.x * c.y + h.y * c.x);
+}
+
+template <bool FADING>
 __global__ void __launch_bounds__(128) conv_link_tx_kernel(const Params p)
 {
     extern __shared__ float2 s_cst[];
@@ -111,6 +131,21 @@ __global__ void __launch_bounds__(128) conv_link_tx_kernel(const Params p)
     int nacc = 0;
     int64_t sym = s0;
     float2 spare = make_float2(0.f, 0.f);
+    float2 hspare = make_float2(0.f, 0.f);                   // fading: the gain of the odd symbol of a pair
+    // fading: the gain of symbol s (pairs share a Philox block like the noise), written to h; returns h * c
+    auto fade = [&](int64_t s, float2 c) -> float2 {
+        float2 h;
+        if ((s & 1) == 0 || s == s0) {
+            const uint4 r = philox4x32_10(make_uint4(f_lo, f_hi, (uint32_t)(s >> 1), 5u), p.seed_lo, p.seed_hi);
+            h = fading_gain(p, box_muller(r.x, r.y));
+            hspare = fading_gain(p, box_muller(r.z, r.w));
+            if (s & 1) h = hspare;
+        } else {
+            h = hspare;
+        }
+        p.h[fl * p.nsym + s] = h;
+        return cmul(h, c);
+    };
     while (sym < s1) {
         const uint32_t u = get_bit(i);
         reg = ((reg << 1) | u) & regmask;
@@ -142,7 +177,7 @@ __global__ void __launch_bounds__(128) conv_link_tx_kernel(const Params p)
                 }
                 nz = spare;
             }
-            const float2 c = s_cst[idx];
+            const float2 c = FADING ? fade(sym, s_cst[idx]) : s_cst[idx];
             y[sym] = make_float2(fmaf(p.sigma, nz.x, c.x), fmaf(p.sigma, nz.y, c.y));
             ++sym;
         }
@@ -165,7 +200,7 @@ __global__ void __launch_bounds__(128) conv_link_tx_kernel(const Params p)
 //   * message bytes leave as 16-byte stores (4 bits -> 4 bytes by one multiply), symbols as 16-byte stores (the two symbols
 //     that share a Philox noise block).
 // ------------------------------------------------------------------------------------------------
-template <int NB>
+template <int NB, bool FADING>
 __global__ void __launch_bounds__(128) conv_link_tx_fast_kernel(const Params p)
 {
     constexpr int H = NB / 2;                    // information bits per symbol
@@ -220,7 +255,14 @@ __global__ void __launch_bounds__(128) conv_link_tx_fast_kernel(const Params p)
             const float2 n0 = box_muller(r.x, r.y), n1 = box_muller(r.z, r.w);
             const uint32_t k0 = ((c0 >> (H * s2)) & ((1u << H) - 1u)) | (((c1 >> (H * s2)) & ((1u << H) - 1u)) << H);
             const uint32_t k1 = ((c0 >> (H * (s2 + 1))) & ((1u << H) - 1u)) | (((c1 >> (H * (s2 + 1))) & ((1u << H) - 1u)) << H);
-            const float2 a0 = s_map[k0], a1 = s_map[k1];
+            float2 a0 = s_map[k0], a1 = s_map[k1];
+            if (FADING) {
+                const uint4 rh = philox4x32_10(make_uint4(f_lo, f_hi, gs >> 1, 5u), p.seed_lo, p.seed_hi);
+                const float2 h0 = fading_gain(p, box_muller(rh.x, rh.y)), h1 = fading_gain(p, box_muller(rh.z, rh.w));
+                *reinterpret_cast<float4 *>(p.h + (y - p.y) + sym) = make_float4(h0.x, h0.y, h1.x, h1.y);
+                a0 = cmul(h0, a0);
+                a1 = cmul(h1, a1);
+            }
             *reinterpret_cast<float4 *>(y + sym) = make_float4(fmaf(p.sigma, n0.x, a0.x), fmaf(p.sigma, n0.y, a0.y),
                                                                fmaf(p.sigma, n1.x, a1.x), fmaf(p.sigma, n1.y, a1.y));
         }
@@ -231,11 +273,15 @@ static int gcd_int(int a, int b) { return b ? gcd_int(b, a % b) : a; }
 
 }  // namespace txlink
 
+// h_dev == nullptr: AWGN; otherwise flat fading with mean gain (los_re, los_im) and scattered power nlos_var
 static int conv_link_tx_impl(const cpbTrellis *t, const cpbModem *m, int64_t frames, int64_t frame_bits, uint64_t seed,
                              int64_t first_frame, float noise_sigma, const int32_t *punct_vec, int punct_len,
-                             uint8_t *msg_dev, float *y_dev, void *stream)
+                             uint8_t *msg_dev, float *y_dev, float *h_dev, float los_re, float los_im, float nlos_var,
+                             void *stream)
 {
     if (!t || !m || frames < 0 || frame_bits < 1 || first_frame < 0) return CPB_EINVAL;
+    if (h_dev && !(nlos_var >= 0.0f && std::isfinite(nlos_var) && std::isfinite(los_re) && std::isfinite(los_im)))
+        return CPB_EINVAL;
     if (frames == 0) return CPB_OK;
     if (!msg_dev || !y_dev) return CPB_EINVAL;
     int k, n, S;
@@ -295,23 +341,37 @@ static int conv_link_tx_impl(const cpbTrellis *t, const cpbModem *m, int64_t fra
     p.cst = reinterpret_cast<const float2 *>(cst);
     p.msg = msg_dev;
     p.y = reinterpret_cast<float2 *>(y_dev);
+    p.h = reinterpret_cast<float2 *>(h_dev);
+    p.los_re = los_re; p.los_im = los_im;
+    p.nlos_std = (float)std::sqrt(0.5 * (double)nlos_var);
+    const bool fading = h_dev != nullptr;
     // word-parallel kernel: n = 2, no puncturing, 2 / 4 / 8 bits per symbol, whole 128-bit message blocks, 16-byte aligned rows
     const bool fast = !punct_vec && n == 2 && (nb == 2 || nb == 4 || nb == 8) && Mc == (1 << nb) && (frame_bits % 128) == 0 &&
                       mem >= 1 && mem < 32 && (reinterpret_cast<uintptr_t>(msg_dev) & 15) == 0 &&
-                      (reinterpret_cast<uintptr_t>(y_dev) & 15) == 0 && !option(CPB_OPT_TX_FORCE_GENERIC);
+                      (reinterpret_cast<uintptr_t>(y_dev) & 15) == 0 && (reinterpret_cast<uintptr_t>(h_dev) & 15) == 0 &&
+                      !option(CPB_OPT_TX_FORCE_GENERIC);
     if (fast) {
         p.chunks = frame_bits / 128;
         const int64_t threads = frames * p.chunks;
         const unsigned grid = (unsigned)ceil_div(threads, 128);
-        if (nb == 2) txlink::conv_link_tx_fast_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(p);
-        else if (nb == 4) txlink::conv_link_tx_fast_kernel<4><<<grid, 128, 0, (cudaStream_t)stream>>>(p);
-        else txlink::conv_link_tx_fast_kernel<8><<<grid, 128, 0, (cudaStream_t)stream>>>(p);
+        cudaStream_t st = (cudaStream_t)stream;
+        if (fading) {
+            if (nb == 2) txlink::conv_link_tx_fast_kernel<2, true><<<grid, 128, 0, st>>>(p);
+            else if (nb == 4) txlink::conv_link_tx_fast_kernel<4, true><<<grid, 128, 0, st>>>(p);
+            else txlink::conv_link_tx_fast_kernel<8, true><<<grid, 128, 0, st>>>(p);
+        } else {
+            if (nb == 2) txlink::conv_link_tx_fast_kernel<2, false><<<grid, 128, 0, st>>>(p);
+            else if (nb == 4) txlink::conv_link_tx_fast_kernel<4, false><<<grid, 128, 0, st>>>(p);
+            else txlink::conv_link_tx_fast_kernel<8, false><<<grid, 128, 0, st>>>(p);
+        }
         CPB_LAUNCH_CHECK();
         return CPB_OK;
     }
     const int64_t threads = frames * p.chunks;
     const unsigned grid = (unsigned)ceil_div(threads, 128);
-    txlink::conv_link_tx_kernel<<<grid, 128, (size_t)Mc * sizeof(float2), (cudaStream_t)stream>>>(p);
+    const size_t smem = (size_t)Mc * sizeof(float2);
+    if (fading) txlink::conv_link_tx_kernel<true><<<grid, 128, smem, (cudaStream_t)stream>>>(p);
+    else txlink::conv_link_tx_kernel<false><<<grid, 128, smem, (cudaStream_t)stream>>>(p);
     CPB_LAUNCH_CHECK();
     return CPB_OK;
 }
@@ -320,7 +380,8 @@ extern "C" int cpb_conv_link_tx(const cpbTrellis *t, const cpbModem *m, int64_t 
                                 uint64_t seed, int64_t first_frame, float noise_sigma, uint8_t *msg_dev, float *y_dev,
                                 void *stream)
 {
-    return conv_link_tx_impl(t, m, frames, frame_bits, seed, first_frame, noise_sigma, nullptr, 0, msg_dev, y_dev, stream);
+    return conv_link_tx_impl(t, m, frames, frame_bits, seed, first_frame, noise_sigma, nullptr, 0, msg_dev, y_dev, nullptr,
+                             0.0f, 0.0f, 0.0f, stream);
 }
 
 extern "C" int cpb_conv_link_tx_punctured(const cpbTrellis *t, const cpbModem *m, int64_t frames, int64_t frame_bits,
@@ -330,5 +391,15 @@ extern "C" int cpb_conv_link_tx_punctured(const cpbTrellis *t, const cpbModem *m
 {
     if (!punct_vec_host) return CPB_EINVAL;
     return conv_link_tx_impl(t, m, frames, frame_bits, seed, first_frame, noise_sigma, punct_vec_host, punct_len, msg_dev,
-                             y_dev, stream);
+                             y_dev, nullptr, 0.0f, 0.0f, 0.0f, stream);
+}
+
+extern "C" int cpb_conv_link_tx_fading(const cpbTrellis *t, const cpbModem *m, int64_t frames, int64_t frame_bits,
+                                       uint64_t seed, int64_t first_frame, float noise_sigma, float los_re, float los_im,
+                                       float nlos_var, const int32_t *punct_vec_host, int punct_len, uint8_t *msg_dev,
+                                       float *y_dev, float *h_dev, void *stream)
+{
+    if (!h_dev && frames > 0) return CPB_EINVAL;
+    return conv_link_tx_impl(t, m, frames, frame_bits, seed, first_frame, noise_sigma, punct_vec_host, punct_len, msg_dev,
+                             y_dev, h_dev, los_re, los_im, nlos_var, stream);
 }

@@ -5,12 +5,14 @@
   package's `Modem.demodulate` and `viterbi_decode`).
 * `AwgnSisoChannel` is the one channel convention the decoding path needs to synthesise its inputs
   (commpy/channels.py:53,74: `noise_std = sqrt((isComplex+1)*nb_tx*Es / (rate*10^(SNR/10)))`, complex noise
-  `(N(0,1) + jN(0,1)) * noise_std * 0.5`).  Fading / MIMO channels are out of scope.
+  `(N(0,1) + jN(0,1)) * noise_std * 0.5`).  Host-side fading channels are in `channels`.
 * `ConvLinkGPU` is the batched form for config C5: random bits -> convolutional encoder -> Modem.modulate ->
   AWGN generated on the device by one CUDA kernel (`conv_link_tx` -> cpb_conv_link_tx, counter-based Philox
   randomness keyed by the GLOBAL frame index), then this package's demapper, Viterbi decoder and error
   counter; frames shard over ranks and the error counters are all-reduced so every rank takes the same
-  stop decision (`links.py:313`).
+  stop decision (`links.py:313`).  With `fading_param` the batched link runs over SISO flat fading instead
+  (`conv_link_tx_fading` -> cpb_conv_link_tx_fading, one gain per symbol as `channels.SISOFlatChannel` draws them), and
+  the demapper uses the gains (cpb_demod_soft_csi / cpb_demod_hard_csi).
 """
 import math
 from fractions import Fraction
@@ -20,7 +22,8 @@ import numpy as np
 
 from . import _lib, parallel
 
-__all__ = ["link_performance", "LinkModel", "AwgnSisoChannel", "ConvLinkGPU", "conv_link_tx", "idd_decoder"]
+__all__ = ["link_performance", "LinkModel", "AwgnSisoChannel", "ConvLinkGPU", "conv_link_tx", "conv_link_tx_fading",
+           "idd_decoder"]
 
 
 class AwgnSisoChannel:
@@ -242,6 +245,47 @@ def conv_link_tx(trellis, modem, frames, frame_bits, seed, first_frame, noise_si
     return msg, y
 
 
+def _fading(fading_param):
+    """(mean gain, scattered power) of a SISOFlatChannel fading_param, checked like the reference checks it (ValueError when
+    the channel would add or remove energy); a real-valued channel raises NotImplementedError (the device link is complex
+    baseband)."""
+    from .channels import SISOFlatChannel
+    ch = SISOFlatChannel(fading_param=fading_param)
+    if not ch.isComplex:
+        raise NotImplementedError("the GPU link is complex baseband: fading_param[0] must be complex, e.g. (0j, 1)")
+    return complex(fading_param[0]), float(np.real(fading_param[1]))
+
+
+def conv_link_tx_fading(trellis, modem, frames, frame_bits, seed, first_frame, noise_sigma, fading_param, puncture=None):
+    """`conv_link_tx` over SISO flat fading (SISOFlatChannel, channels.py:176-221): each symbol c is received as
+    y = h c + noise_sigma * (N(0,1) + jN(0,1)) with its own gain h = fading_param[0] + sqrt(fading_param[1] / 2) *
+    (N(0,1) + jN(0,1)), e.g. (0j, 1) for Rayleigh and (m, 1 - |m|^2) for Rician fading.  The message and the noise are
+    the streams of `conv_link_tx` (at fading_param = (1 + 0j, 0) the outputs are identical to it).
+
+    Returns (msg uint8 (frames, frame_bits), y complex64 (frames, nsym), h complex64 (frames, nsym)) as CUDA tensors."""
+    import ctypes as C
+    from .channelcoding.convcode import _trellis_handle
+    mean, nlos = _fading(fading_param)
+    torch = _lib.require_cuda()
+    nb = int(modem.num_bits_symbol)
+    kept = kept_bits(int(trellis.n) * int(frame_bits), puncture)
+    if kept % nb:
+        raise ValueError("the (punctured) coded bits of a frame must fill whole symbols")
+    nsym = kept // nb
+    msg = torch.empty((int(frames), int(frame_bits)), dtype=torch.uint8, device="cuda")
+    y = torch.empty((int(frames), nsym), dtype=torch.complex64, device="cuda")
+    h = torch.empty((int(frames), nsym), dtype=torch.complex64, device="cuda")
+    pv = None if puncture is None else np.ascontiguousarray(puncture, dtype=np.int32)
+    rc = _lib.load().cpb_conv_link_tx_fading(_trellis_handle(trellis), modem._handle(), C.c_int64(int(frames)),
+                                             C.c_int64(int(frame_bits)), C.c_uint64(int(seed) & ((1 << 64) - 1)),
+                                             C.c_int64(int(first_frame)), C.c_float(float(noise_sigma)),
+                                             C.c_float(mean.real), C.c_float(mean.imag), C.c_float(nlos), _lib.ptr(pv),
+                                             0 if pv is None else int(len(pv)), _lib.ptr(msg), _lib.ptr(y), _lib.ptr(h),
+                                             _lib.stream_ptr(torch))
+    _lib.check(rc, "conv_link_tx_fading")
+    return msg, y, h
+
+
 def kept_bits(n_coded, puncture):
     """how many of n_coded bits puncturing(message, puncture) keeps (convcode.py:752-774)"""
     if puncture is None:
@@ -255,10 +299,15 @@ class ConvLinkGPU:
 
     Parameters: `trellis` (k=1 feed-forward, e.g. the K=7 (0o133,0o171) code), `modem` (commpy_b200 Modem),
     `frame_bits` information bits per frame ('cont' termination), `frames_per_batch` frames decoded per step and rank.
+    `fading_param` (a SISOFlatChannel fading_param with a complex mean, e.g. (0j, 1) for Rayleigh): the link runs over
+    i.i.d. flat fading, one gain per symbol, known to the receiver's demapper; None: AWGN.
     """
 
     def __init__(self, trellis, modem, frame_bits=4096, frames_per_batch=4096, decoding_type="soft", tb_depth=None, seed=0,
-                 puncture=None):
+                 puncture=None, fading_param=None):
+        self.fading_param = fading_param
+        if fading_param is not None:
+            _fading(fading_param)
         taps = _ff_taps(trellis)
         if taps is None:
             raise NotImplementedError("ConvLinkGPU generates frames on the device for k=1 feed-forward codes only")
@@ -285,23 +334,28 @@ class ConvLinkGPU:
         return math.sqrt(2 * self.modem.Es / (float(self.rate) * 10 ** (snr_db / 10)))
 
     def make_batch(self, snr_db, batch_index, torch=None):
-        """(msg bits, received symbols, noise_var) for one batch of this rank -- everything stays on the device.
+        """(msg bits, received symbols, noise_var) for one batch of this rank -- everything stays on the device -- and,
+        over fading, the channel gains as a fourth element.
         Batch `batch_index` of rank r covers the global frames [(batch_index*world + r) * frames, ... + frames)."""
         rank, world, _ = parallel.world()
         first = parallel.batch_first_frame(batch_index, self.frames, rank, max(world, 1))
         ns = self.noise_std(snr_db)
+        if self.fading_param is not None:
+            msg, y, h = conv_link_tx_fading(self.trellis, self.modem, self.frames, self.frame_bits, self.seed, first, 0.5 * ns,
+                                            self.fading_param, self.puncture)
+            return msg, y, ns ** 2, h
         msg, y = conv_link_tx(self.trellis, self.modem, self.frames, self.frame_bits, self.seed, first, 0.5 * ns,
                               self.puncture)
         return msg, y, ns ** 2                                                                     # links.py:329
 
     # -- RX chain: this package's kernels -------------------------------------------------------------
-    def receive_decode_count(self, msg, y, noise_var, counters, torch):
+    def receive_decode_count(self, msg, y, noise_var, counters, torch, channel_gains=None):
         import ctypes as C
         from .channelcoding import viterbi_decode_batch
         if self.decoding_type == "soft":
-            rx = self.modem.demodulate_batch(y, "soft", noise_var)
+            rx = self.modem.demodulate_batch(y, "soft", noise_var, channel_gains)
         else:
-            rx = self.modem.demodulate_batch(y, "hard")
+            rx = self.modem.demodulate_batch(y, "hard", channel_gains=channel_gains)
         if self.puncture is None:
             dec = viterbi_decode_batch(rx, self.trellis, self.tb_depth, self.decoding_type)
         else:
@@ -354,10 +408,10 @@ class ConvLinkGPU:
             hist = []                                                        # (device snapshot, pinned copy, event)
             bits_known = 0
             while True:
-                msg, y, nv = self.make_batch(float(snr), batch_index, torch)
+                msg, y, nv, *gains = self.make_batch(float(snr), batch_index, torch)
                 batch_index += 1
                 local = torch.zeros(3, dtype=torch.int64, device="cuda")
-                self.receive_decode_count(msg, y, nv, local, torch)
+                self.receive_decode_count(msg, y, nv, local, torch, *gains)
                 local[2] = msg.numel()
                 parallel.allreduce_counters(local)
                 tot = tot + local

@@ -82,11 +82,16 @@ class Modem:
             self._handles[dev] = box
         return box.ptr
 
-    def demodulate_batch(self, input_symbols, demod_type, noise_var=0):
+    def demodulate_batch(self, input_symbols, demod_type, noise_var=0, channel_gains=None):
         """GPU demapper on a torch CUDA complex64 tensor (or numpy complex array) of any shape.
 
         Returns a torch CUDA tensor shaped input.shape + (num_bits_symbol,) flattened on the last two axes:
-        float32 LLRs ('soft') or uint8 bits ('hard')."""
+        float32 LLRs ('soft') or uint8 bits ('hard').
+
+        `channel_gains` (a scalar, or an array or tensor broadcastable to the symbols): the flat-fading gain h of each
+        symbol, known to the receiver.  The distances become |y - h c|^2, i.e. the reference's
+        demodulate(y / h, 'soft', noise_var / |h|^2) symbol by symbol (cpb_demod_soft_csi / cpb_demod_hard_csi); LLRs are
+        finite in deep fades and 0 where h = 0.  None: the AWGN demapper."""
         torch = _lib.require_cuda()
         if demod_type not in ("hard", "soft"):
             raise ValueError('demod_type must be "hard" or "soft"')
@@ -101,15 +106,24 @@ class Modem:
         nb = self.num_bits_symbol
         yr = torch.view_as_real(y)
         lib = _lib.load()
+        h = None if channel_gains is None else _gains_like(channel_gains, y, torch)
         if demod_type == "soft":
             if not noise_var > 0:
                 raise ValueError("noise_var must be positive for soft demodulation")
             out = torch.empty((nsym * nb,), dtype=torch.float32, device=y.device)
-            rc = lib.cpb_demod_soft(self._handle(), _lib.ptr(yr), C.c_int64(nsym), C.c_float(noise_var), _lib.ptr(out),
-                                    _lib.stream_ptr(torch))
+            if h is None:
+                rc = lib.cpb_demod_soft(self._handle(), _lib.ptr(yr), C.c_int64(nsym), C.c_float(noise_var), _lib.ptr(out),
+                                        _lib.stream_ptr(torch))
+            else:
+                rc = lib.cpb_demod_soft_csi(self._handle(), _lib.ptr(yr), _lib.ptr(h), C.c_int64(nsym), C.c_float(noise_var),
+                                            _lib.ptr(out), _lib.stream_ptr(torch))
         else:
             out = torch.empty((nsym * nb,), dtype=torch.uint8, device=y.device)
-            rc = lib.cpb_demod_hard(self._handle(), _lib.ptr(yr), C.c_int64(nsym), _lib.ptr(out), _lib.stream_ptr(torch))
+            if h is None:
+                rc = lib.cpb_demod_hard(self._handle(), _lib.ptr(yr), C.c_int64(nsym), _lib.ptr(out), _lib.stream_ptr(torch))
+            else:
+                rc = lib.cpb_demod_hard_csi(self._handle(), _lib.ptr(yr), _lib.ptr(h), C.c_int64(nsym), _lib.ptr(out),
+                                            _lib.stream_ptr(torch))
         _lib.check(rc, "demodulate")
         return out.reshape(tuple(y.shape[:-1]) + (y.shape[-1] * nb,)) if y.dim() > 1 else out
 
@@ -126,16 +140,41 @@ class Modem:
         _lib.check(rc, "demodulate")
         return out.reshape(tuple(y.shape[:-1]) + (y.shape[-1] * self.num_bits_symbol,)) if y.ndim > 1 else out
 
-    def demodulate(self, input_symbols, demod_type, noise_var=0):
+    def demodulate(self, input_symbols, demod_type, noise_var=0, channel_gains=None):
         """Drop-in for Modem.demodulate (modulation.py:100-141).
 
         'hard': nearest constellation point -> its bits (int8).  'soft': exact log-sum-exp LLRs
         log(sum_{bit=1} exp(-|y-c|^2/noise_var) / sum_{bit=0} ...), float64 array, MSB first per symbol.
-        Computed in float32 on the GPU (relative error ~1e-4); finite where the reference under/overflows."""
+        Computed in float32 on the GPU (relative error ~1e-4); finite where the reference under/overflows.
+        `channel_gains`: per-symbol flat-fading gains h (see `demodulate_batch`); a fading receiver for LinkModel is
+        `lambda y, h, c, nv: modem.demodulate(y, 'soft', nv, channel_gains=h)`."""
+        if channel_gains is not None:
+            y = np.atleast_1d(np.asarray(input_symbols))
+            try:
+                h = np.broadcast_to(np.asarray(channel_gains), y.shape)
+            except ValueError:
+                raise ValueError("channel_gains of shape %s does not broadcast to the symbols' shape %s"
+                                 % (np.shape(channel_gains), y.shape)) from None
+            out = self.demodulate_batch(y.reshape(-1), demod_type, noise_var, h.reshape(-1)).cpu().numpy()
+            return out.astype(np.float64) if demod_type == "soft" else out.astype(np.int8)
         if demod_type == "soft":
             return self.demodulate_soft_host(np.atleast_1d(np.asarray(input_symbols)).reshape(-1), noise_var).astype(np.float64)
         out = self.demodulate_batch(np.atleast_1d(np.asarray(input_symbols)).reshape(-1), demod_type, noise_var)
         return out.cpu().numpy().astype(np.int8)
+
+
+def _gains_like(channel_gains, y, torch):
+    """per-symbol gains as a contiguous complex64 tensor of y's shape on y's device"""
+    if hasattr(channel_gains, "data_ptr"):
+        h = channel_gains.to(device=y.device, dtype=torch.complex64)
+    else:
+        h = torch.from_numpy(np.ascontiguousarray(channel_gains, dtype=np.complex64)).to(y.device)
+    try:
+        h = torch.broadcast_to(h, y.shape)
+    except RuntimeError:
+        raise ValueError("channel_gains of shape %s does not broadcast to the symbols' shape %s"
+                         % (tuple(h.shape), tuple(y.shape))) from None
+    return torch.view_as_real(h.contiguous())
 
 
 class PSKModem(Modem):

@@ -48,12 +48,14 @@ class Wifi80211:
     def _get_trellis():
         return cc.Trellis(Wifi80211.memory, Wifi80211.generator_matrix)
 
-    def link_performance_gpu(self, SNRs, send_max, err_min, send_chunk=4096, frames_per_batch=4096, seed=0, stop_early=True):
+    def link_performance_gpu(self, SNRs, send_max, err_min, send_chunk=4096, frames_per_batch=4096, seed=0, stop_early=True,
+                             fading_param=None):
         """The same MCS over an AWGN SISO channel, batched on the GPU(s): frames are generated, punctured, mapped and
         disturbed on the device (cpb_conv_link_tx[_punctured]), demapped (cpb_demod_soft) and decoded with the depuncturing
         fused into the Viterbi kernel's load (cpb_viterbi_decode_punctured).  `send_chunk` information bits per frame
         (rounded down so that the punctured frame fills whole symbols and whole puncturing periods).  Returns the BER per
-        SNR like `ConvLinkGPU.link_performance`."""
+        SNR like `ConvLinkGPU.link_performance`.  `fading_param` (e.g. (0j, 1), Rayleigh): SISO flat fading instead of AWGN,
+        with a demapper that knows the gains (see `ConvLinkGPU`)."""
         num, den = self._get_coding()
         modem = self.get_modem()
         pattern = Wifi80211._get_puncture_matrix(num, den)
@@ -63,7 +65,7 @@ class Wifi80211:
             unit += 1
         frame_bits = max(unit, (int(send_chunk) // unit) * unit)
         self.gpu_link = lk.ConvLinkGPU(Wifi80211._get_trellis(), modem, frame_bits=frame_bits, frames_per_batch=frames_per_batch,
-                                       decoding_type="soft", seed=seed, puncture=pattern)
+                                       decoding_type="soft", seed=seed, puncture=pattern, fading_param=fading_param)
         return self.gpu_link.link_performance(SNRs, send_max, err_min, stop_early=stop_early)
 
     def link_performance(self, channel, SNRs, tx_max, err_min, send_chunk=None, frame_aggregation=1, receiver=None,

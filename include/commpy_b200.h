@@ -194,6 +194,16 @@ int cpb_demod_soft(const cpbModem *m, const float *y_dev, int64_t n_sym, float n
 int cpb_demod_soft_host(const cpbModem *m, const float *y_host, int64_t n_sym, float noise_var, float *llr_host);
 /* bits_dev: n_sym x log2(M) uint8, nearest point (first minimum), MSB first (:121-123). */
 int cpb_demod_hard(const cpbModem *m, const float *y_dev, int64_t n_sym, uint8_t *bits_dev, void *stream);
+/*
+ * Channel-aware forms for flat fading: h_dev holds n_sym complex64 gains, one per symbol, and the distances are
+ * |y - h c_k|^2.  The LLRs equal the reference's demodulate(y/h, 'soft', noise_var/|h|^2) symbol by symbol, without
+ * dividing by h: finite in deep fades, exactly 0 where |h|^2 is 0 (hard decision: index 0 there).  With h = 1 the output
+ * equals cpb_demod_soft / cpb_demod_hard bit for bit.
+ */
+int cpb_demod_soft_csi(const cpbModem *m, const float *y_dev, const float *h_dev, int64_t n_sym, float noise_var,
+                       float *llr_dev, void *stream);
+int cpb_demod_hard_csi(const cpbModem *m, const float *y_dev, const float *h_dev, int64_t n_sym, uint8_t *bits_dev,
+                       void *stream);
 
 /* ---- error counting: commpy/links.py:335-337 (and :253-256) ------------------------------------- */
 /* counters_dev[0] += # differing bits, counters_dev[1] += # frames with >= 1 differing bit (int64, device). */
@@ -219,6 +229,14 @@ int cpb_conv_link_tx_punctured(const cpbTrellis *t, const cpbModem *m, int64_t f
                                uint64_t seed, int64_t first_frame, float noise_sigma,
                                const int32_t *punct_vec_host, int punct_len, uint8_t *msg_dev, float *y_dev,
                                void *stream);
+/* The same over a flat-fading SISO channel (SISOFlatChannel, channels.py:176-221): symbol s gets its own gain
+ * h = (los_re + j los_im) + sqrt(nlos_var / 2) (N(0,1) + j N(0,1)) (Philox counter word 5) and y = h * point + noise, the
+ * noise stream being that of cpb_conv_link_tx.  h_dev: frames x nsym complex64, laid out like y_dev.  punct_vec_host may be
+ * NULL (no puncturing).  With los = 1, nlos_var = 0 the message and y equal cpb_conv_link_tx[_punctured] bit for bit. */
+int cpb_conv_link_tx_fading(const cpbTrellis *t, const cpbModem *m, int64_t frames, int64_t frame_bits, uint64_t seed,
+                            int64_t first_frame, float noise_sigma, float los_re, float los_im, float nlos_var,
+                            const int32_t *punct_vec_host, int punct_len,
+                            uint8_t *msg_dev, float *y_dev, float *h_dev, void *stream);
 
 /* ---- transmit side of a turbo-coded BPSK-AWGN link: commpy/channelcoding/turbo.py:14-59 (turbo_encode) + mapper + AWGN ---- */
 /*

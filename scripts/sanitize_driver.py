@@ -57,5 +57,18 @@ link = ConvLinkGPU(tr, QAMModem(16), frame_bits=512, frames_per_batch=64, decodi
 link.link_performance([9.0], send_max=100000, err_min=10 ** 9)
 link = ConvLinkGPU(helpers.k7_wifi_quirk(), QAMModem(256), frame_bits=600, frames_per_batch=64, decoding_type="soft", seed=1, puncture=pv)
 link.link_performance([27.0], send_max=100000, err_min=10 ** 9)
+# flat fading: CSI demapper (separable, general, hard, h = 0 included), fading TX (word-parallel, bit-serial, punctured)
+h = torch.view_as_complex(torch.randn(5000, 2, device="cuda"))
+h[::50] = 0
+QAMModem(64).demodulate_batch(y, "soft", 1.5, channel_gains=h)
+PSKModem(8).demodulate_batch(y, "soft", 0.5, channel_gains=h)
+QAMModem(16).demodulate_batch(y, "hard", channel_gains=h)
+link = ConvLinkGPU(tr, QAMModem(16), frame_bits=512, frames_per_batch=64, decoding_type="soft", seed=1, fading_param=(0j, 1))
+link.link_performance([12.0], send_max=100000, err_min=10 ** 9)
+link = ConvLinkGPU(tr, QAMModem(4), frame_bits=200, frames_per_batch=64, decoding_type="hard", seed=1, fading_param=(0j, 1))
+link.link_performance([12.0], send_max=30000, err_min=10 ** 9)
+link = ConvLinkGPU(helpers.k7_wifi_quirk(), QAMModem(16), frame_bits=600, frames_per_batch=64, decoding_type="soft", seed=1,
+                   puncture=pv, fading_param=(0.6 + 0j, 0.64))
+link.link_performance([20.0], send_max=100000, err_min=10 ** 9)
 torch.cuda.synchronize()
 print("sanitize driver ok")
