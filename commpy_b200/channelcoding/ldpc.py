@@ -177,8 +177,9 @@ def ldpc_bp_decode(llr_vec, ldpc_code_params, decoder_algorithm, n_iters, precis
     `llr_vec` (1-D, one or several blocks back to back) is clipped in place to +-500 like the reference
     (:186).  With the default precision='fp64' the GPU reproduces the float64 reference bit for bit
     (decisions AND out_llrs); precision='fp32' is the throughput mode.  Returns (dec_word int8, out_llrs) with
-    one block per column, squeezed (:251-254).  'SPA' (sum-product, :209-227) agrees with the reference to rounding
-    (~1e-12 on out_llrs in fp64), 'MSA' exactly; any other name raises NameError as the reference does (:239-240).
+    one block per column, squeezed (:251-254).  'SPA' (sum-product, :209-227) agrees with the reference within the
+    conditioning of its check node (messages near the +-500 saturation knee may round either way; DESIGN.md section 4.4),
+    'MSA' exactly; any other name raises NameError as the reference does (:239-240).
     """
     if decoder_algorithm not in ("MSA", "SPA"):
         raise NameError('Please input a valid decoder_algorithm string (meanning "SPA" or "MSA").')

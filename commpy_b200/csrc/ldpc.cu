@@ -479,9 +479,26 @@ static size_t smem_bytes(int maxdeg, int FT)
 
 }  // namespace bulk
 
+// The NaN an x86 CPU produces for 0 * inf (sign bit set), and the quiet NaN with a clear sign bit.
+template <typename T> __device__ __forceinline__ T x86_default_nan();
+template <> __device__ __forceinline__ float x86_default_nan<float>() { return __int_as_float(0xffc00000u); }
+template <> __device__ __forceinline__ double x86_default_nan<double>() { return __longlong_as_double(0xfff8000000000000ull); }
+template <typename T> __device__ __forceinline__ T positive_nan();
+template <> __device__ __forceinline__ float positive_nan<float>() { return __int_as_float(0x7fc00000u); }
+template <> __device__ __forceinline__ double positive_nan<double>() { return __longlong_as_double(0x7ff8000000000000ull); }
+
 // Sum-product check node (ldpc.py:209-227): t = tanh(Q/2), R_ij = 2 atanh(clip((prod_row t) / t_ij, -1, 1)) clipped to
 // +-500.  Same formula as the reference (product of the whole row divided by the edge's own factor); the product is
-// formed directly instead of through exp2(sum(log2(complex))) so results agree to rounding (~1e-13), not bit for bit.
+// formed directly instead of through exp2(sum(log2(complex))).  Q_ij is formed in the message type T, everything after
+// it in double whatever T is, and R is rounded to T once: an fp32 message can then take any value up to the reference's
+// saturation knee 2 atanh(1 - 2^-53) ~ 37.4 (in float the knee would be 2 atanh(1 - 2^-24) ~ 17.3, and every message
+// between 17.3 and 37.4 would jump to 500).  Conditioning: with x = prod/t_ij computed to a relative error rho
+// (~3 deg eps here, eps = 2^-53, plus the reference's own log2/exp2 error), |dR| <= 2 atanh(|x|(1+rho)) - 2 atanh(|x|)
+// ~ 2 rho |x| cosh^2(R/2), so a message near the knee may legitimately come out as ~37 in one and 500 in the other.
+// Exact zeros: tanh(+-0) = +-0 makes the product +-0 (sign = parity of the sign bits, as the reference's complex log
+// counts arg(-0) = pi) and the zero edge's own message (1/+-0) * +-0 = NaN.  On x86 that NaN has its sign bit set, which
+// the reference's decision signbit() turns into a 1; the kernel writes the same NaN, and vn_spa_kernel keeps its sign.
+// A NaN that enters through Q has passed numpy's tanh, whose NaN is positive: the kernel writes a positive NaN then.
 template <typename T>
 __global__ void __launch_bounds__(256) cn_spa_kernel(const int32_t *__restrict__ row_ptr, const int32_t *__restrict__ col_idx,
                                                      int m, int64_t F, int iter, const T *__restrict__ post,
@@ -502,10 +519,10 @@ __global__ void __launch_bounds__(256) cn_spa_kernel(const int32_t *__restrict__
     for (int v = 0; v < V; ++v) { act[v] = st.done[f + v] == 0; any |= act[v]; }
     if (!any) return;
     const int e0 = __ldg(&row_ptr[i]), e1 = __ldg(&row_ptr[i + 1]);
-    T prod[V];
+    double prod[V];
     int par[V];
 #pragma unroll
-    for (int v = 0; v < V; ++v) { prod[v] = (T)1; par[v] = 0; }
+    for (int v = 0; v < V; ++v) { prod[v] = 1.0; par[v] = 0; }
     for (int e = e0; e < e1; ++e) {
         const int c = __ldg(&col_idx[e]);
         const VT p = *reinterpret_cast<const VT *>(post + (int64_t)c * F + f);
@@ -513,7 +530,8 @@ __global__ void __launch_bounds__(256) cn_spa_kernel(const int32_t *__restrict__
 #pragma unroll
         for (int v = 0; v < V; ++v) {
             par[v] ^= signbit(p.v[v]) ? 1 : 0;
-            prod[v] *= tanh((p.v[v] - r.v[v]) * (T)0.5);
+            const T q = p.v[v] - r.v[v];                                 // Q_ij, ldpc.py:244-245
+            prod[v] *= tanh((double)q * 0.5);
         }
     }
 #pragma unroll
@@ -525,22 +543,28 @@ __global__ void __launch_bounds__(256) cn_spa_kernel(const int32_t *__restrict__
         VT r = *reinterpret_cast<const VT *>(Rf + (int64_t)e * RS);
 #pragma unroll
         for (int v = 0; v < V; ++v) {
-            const T t = tanh((p.v[v] - r.v[v]) * (T)0.5);
-            T x = ((T)1 / t) * prod[v];
-            x = x > (T)1 ? (T)1 : (x < (T)-1 ? (T)-1 : x);           // NaN (a zero LLR in the row) passes through, as in numpy
-            x = atanh(x) * (T)2;
-            x = x > (T)500 ? (T)500 : (x < (T)-500 ? (T)-500 : x);
-            if (act[v]) r.v[v] = x;
+            const T q = p.v[v] - r.v[v];
+            const double t = tanh((double)q * 0.5);
+            double x = (1.0 / t) * prod[v];
+            x = x > 1.0 ? 1.0 : (x < -1.0 ? -1.0 : x);               // NaN passes through, as in numpy
+            x = atanh(x) * 2.0;
+            x = x > 500.0 ? 500.0 : (x < -500.0 ? -500.0 : x);
+            // a NaN made here ((1/+-0) * +-0) has the sign bit set, one that came in through Q has it clear, whatever
+            // sign the device's tanh/atanh pass on (its tanh keeps the sign of a NaN argument, numpy's does not)
+            const T y = isnan(x) ? (isnan(prod[v]) ? positive_nan<T>() : x86_default_nan<T>()) : (T)x;
+            if (act[v]) r.v[v] = y;
         }
         *reinterpret_cast<VT *>(Rf + (int64_t)e * RS) = r;
     }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256) vn_kernel(const int32_t *__restrict__ col_ptr, const int32_t *__restrict__ col_edge,
-                                                 int n, int64_t F, int iter, const T *__restrict__ llrT,
-                                                 const T *__restrict__ Rbase, T *__restrict__ post, const State st,
-                                                 const RLayout rl)
+// NAN_SIGN: a posterior that is NaN takes the sign bit of the first NaN message of the column, as x86 addition passes
+// a NaN operand through unchanged (the GPU's add returns its own NaN).  Only the sum-product decoder makes NaN messages.
+template <typename T, bool NAN_SIGN>
+__device__ __forceinline__ void vn_body(const int32_t *__restrict__ col_ptr, const int32_t *__restrict__ col_edge,
+                                        int n, int64_t F, int iter, const T *__restrict__ llrT,
+                                        const T *__restrict__ Rbase, T *__restrict__ post, const State st,
+                                        const RLayout rl)
 {
     using VT = typename VecOf<T>::type;
     constexpr int V = VecOf<T>::V;
@@ -567,20 +591,45 @@ __global__ void __launch_bounds__(256) vn_kernel(const int32_t *__restrict__ col
     if (!any) return;
     const int c0 = __ldg(&col_ptr[j]), c1 = __ldg(&col_ptr[j + 1]);
     T tot[V];
+    int nan_sign[V];                            // -1: no NaN message yet, else the sign bit of the first one
 #pragma unroll
-    for (int v = 0; v < V; ++v) tot[v] = (T)0;
+    for (int v = 0; v < V; ++v) { tot[v] = (T)0; nan_sign[v] = -1; }
     for (int q = c0; q < c1; ++q) {             // ascending check index = the reference's summation order
         const int e = __ldg(&col_edge[q]);
         const VT r = *reinterpret_cast<const VT *>(Rf + (int64_t)e * RS);
 #pragma unroll
-        for (int v = 0; v < V; ++v) tot[v] += r.v[v];
+        for (int v = 0; v < V; ++v) {
+            tot[v] += r.v[v];
+            if (NAN_SIGN && nan_sign[v] < 0 && isnan(r.v[v])) nan_sign[v] = signbit(r.v[v]) ? 1 : 0;
+        }
     }
     const VT l = *reinterpret_cast<const VT *>(llrT + (int64_t)j * F + f);
     VT p = *reinterpret_cast<const VT *>(post + (int64_t)j * F + f);
 #pragma unroll
-    for (int v = 0; v < V; ++v)
-        if (act[v]) p.v[v] = tot[v] + l.v[v];                          // ldpc.py:247
+    for (int v = 0; v < V; ++v) {
+        T x = tot[v] + l.v[v];                                          // ldpc.py:247
+        if (NAN_SIGN && nan_sign[v] >= 0) x = copysign(x, nan_sign[v] ? (T)-1 : (T)1);
+        if (act[v]) p.v[v] = x;
+    }
     *reinterpret_cast<VT *>(post + (int64_t)j * F + f) = p;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) vn_kernel(const int32_t *__restrict__ col_ptr, const int32_t *__restrict__ col_edge,
+                                                 int n, int64_t F, int iter, const T *__restrict__ llrT,
+                                                 const T *__restrict__ Rbase, T *__restrict__ post, const State st,
+                                                 const RLayout rl)
+{
+    vn_body<T, false>(col_ptr, col_edge, n, F, iter, llrT, Rbase, post, st, rl);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) vn_spa_kernel(const int32_t *__restrict__ col_ptr, const int32_t *__restrict__ col_edge,
+                                                     int n, int64_t F, int iter, const T *__restrict__ llrT,
+                                                     const T *__restrict__ Rbase, T *__restrict__ post, const State st,
+                                                     const RLayout rl)
+{
+    vn_body<T, true>(col_ptr, col_edge, n, F, iter, llrT, Rbase, post, st, rl);
 }
 
 static size_t state_bytes(int64_t F) { return (size_t)F * sizeof(int32_t) * 3; }
@@ -664,7 +713,8 @@ static int run(const cpbLdpc *h, T *llr, int64_t batch, int n_iters, int spa, ui
             else if (spa) cn_spa_kernel<T><<<cn_blocks, 256, 0, st>>>(h->row_ptr, h->col_idx, h->m, F, it, post, R, s, rl);
             else if (h->max_row_deg <= 8) cn_kernel<T, 8><<<cn_blocks, 256, 0, st>>>(h->row_ptr, h->col_idx, h->m, F, it, post, R, s, rl);
             else cn_kernel<T, 0><<<cn_blocks, 256, 0, st>>>(h->row_ptr, h->col_idx, h->m, F, it, post, R, s, rl);
-            vn_kernel<T><<<vn_blocks, 256, 0, st>>>(h->col_ptr, h->col_edge, h->n, F, it, llrT, R, post, s, rl);
+            if (spa) vn_spa_kernel<T><<<vn_blocks, 256, 0, st>>>(h->col_ptr, h->col_edge, h->n, F, it, llrT, R, post, s, rl);
+            else vn_kernel<T><<<vn_blocks, 256, 0, st>>>(h->col_ptr, h->col_edge, h->n, F, it, llrT, R, post, s, rl);
         }
         store_kernel<T><<<tgrid, 256, 0, st>>>(post, nb, h->n, F, dec + f0 * h->n, out_llr ? out_llr + f0 * h->n : nullptr);
         if (iters_out)

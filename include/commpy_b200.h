@@ -171,8 +171,9 @@ int cpb_ldpc_decode_host(const cpbLdpc *h, int algorithm, void *llr_host, int pr
                          uint8_t *dec_host, void *out_llr_host, int32_t *iters_host);
 
 /* Sum-product variant ('SPA', ldpc.py:209-227): same arguments and schedule; check-node rule
- * R_ij = 2 atanh(clip(prod_row tanh(Q/2) / tanh(Q_ij/2), -1, 1)), clipped to +-500.  Agrees with the reference to
- * rounding (the reference forms the product through complex log2/exp2), not bit for bit. */
+ * R_ij = 2 atanh(clip(prod_row tanh(Q/2) / tanh(Q_ij/2), -1, 1)), clipped to +-500, evaluated in double for both
+ * precisions (fp32 messages saturate at ~37.4, as the reference's do).  Agrees with the reference within the
+ * conditioning of atanh near +-1 (the reference forms the product through complex log2/exp2), not bit for bit. */
 int cpb_ldpc_sumproduct(const cpbLdpc *h, void *llr_dev, int precision, int64_t batch, int n_iters,
                         uint8_t *dec_dev, void *out_llr_dev, int32_t *iters_dev,
                         void *workspace_dev, size_t workspace_bytes, void *stream);
