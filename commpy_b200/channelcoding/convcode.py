@@ -234,75 +234,26 @@ def depuncturing(punctured, punct_vec, shouldbe):
 _MODE_ERR = 'The available decoding types are "hard", "soft" and "unquantized'
 
 
-def _sizes(trellis, n_in):
+def _decoded_bits(trellis, n_in, tb_depth):
+    """Decoded bits L of a frame of n_in coded values; ValueError when tb_depth leaves no complete traceback window."""
     L = int(n_in * (trellis.k / trellis.n))                        # convcode.py:699
     T = int((L + trellis.total_memory) / trellis.k) - 1            # :721
-    return L, T
-
-
-def _check_depth(trellis, L, T, tb_depth):
     D = min(5 * trellis.total_memory, L) if tb_depth is None else int(tb_depth)      # :701-702
     if D < 2 or T < D - 1:
         raise ValueError("tb_depth=%d leaves no complete traceback window for %d trellis steps "
                          "(the reference returns uninitialised memory here)" % (D, T))
-    return D
+    return L
 
 
-def _host_buffer(coded, hard, torch):
-    """numpy array / CPU torch tensor -> (object keeping it alive, pointer source, batch, n_in) in the kernel's dtype."""
-    if hasattr(coded, "data_ptr"):
-        want = torch.uint8 if hard else torch.float32
-        x = coded if coded.dtype == want else coded.to(want)
-        x = x.contiguous()
-        return x, x.shape[0], x.shape[1]
+def _numpy_rows(coded, hard):
+    """numpy rows in the kernel's dtype: uint8 bits (hard decision, values checked) or float32."""
     a = np.asarray(coded)
-    if hard:
-        ai = a if a.dtype == np.uint8 else a.astype(np.int64)          # astype(int): convcode.py:579
-        if ai.size and (ai.min() < 0 or ai.max() > 1):
-            raise ValueError("hard-decision input must contain only 0 and 1")
-        a = np.ascontiguousarray(ai, dtype=np.uint8)
-    else:
-        a = np.ascontiguousarray(a, dtype=np.float32)
-    return a, a.shape[0], a.shape[1]
-
-
-def _viterbi_decode_packed(coded, trellis, tb_depth, out):
-    """Hard decision on bit-packed rows (numpy.packbits order): (batch, n_in/8) uint8 -> (batch, L/8) uint8."""
-    torch = _lib.require_cuda()
-    lib = _lib.load()
-    handle = _trellis_handle(trellis)
-    on_device = hasattr(coded, "data_ptr") and coded.is_cuda
-    if hasattr(coded, "data_ptr"):
-        if coded.dtype != torch.uint8:
-            raise ValueError("packed input must be uint8")
-        x = coded.contiguous()
-    else:
-        x = np.ascontiguousarray(coded)
-        if x.dtype != np.uint8:
-            raise ValueError("packed input must be uint8")
-    batch, nbytes = x.shape
-    n_in = 8 * nbytes
-    L, T = _sizes(trellis, n_in)
-    _check_depth(trellis, L, T, tb_depth)
-    if L % 8:
-        raise NotImplementedError("packed decode needs a whole number of output bytes per frame")
-    if out is None:
-        if on_device:
-            out = torch.empty((batch, L // 8), dtype=torch.uint8, device=x.device)
-        elif hasattr(coded, "data_ptr"):
-            out = torch.empty((batch, L // 8), dtype=torch.uint8)
-        else:
-            out = np.empty((batch, L // 8), np.uint8)
-    else:
-        _check_out(out, (batch, L // 8), x, torch)
-    if on_device:
-        rc = lib.cpb_viterbi_decode_packed(handle, _lib.ptr(x), C.c_int64(batch), C.c_int64(n_in), int(tb_depth or 0),
-                                           _lib.ptr(out), _lib.stream_ptr(torch))
-    else:
-        rc = lib.cpb_viterbi_decode_host_packed(handle, _lib.ptr(x), C.c_int64(batch), C.c_int64(n_in), int(tb_depth or 0),
-                                                _lib.ptr(out))
-    _lib.check(rc, "viterbi_decode (packed)")
-    return out
+    if not hard:
+        return np.ascontiguousarray(a, dtype=np.float32)
+    ai = a if a.dtype == np.uint8 else a.astype(np.int64)          # astype(int): convcode.py:579
+    if ai.size and (ai.min() < 0 or ai.max() > 1):
+        raise ValueError("hard-decision input must contain only 0 and 1")
+    return np.ascontiguousarray(ai, dtype=np.uint8)
 
 
 def _check_out(out, shape, like, torch):
@@ -332,50 +283,51 @@ def viterbi_decode_batch(coded, trellis, tb_depth=None, decoding_type="hard", ou
     """
     if decoding_type not in _lib.VITERBI_MODES:
         raise ValueError(_MODE_ERR)
-    if packed:
-        if decoding_type != "hard":
-            raise ValueError("packed=True is a hard-decision format")
-        if getattr(coded, "ndim", None) != 2 and not (hasattr(coded, "dim") and coded.dim() == 2):
-            raise ValueError("coded must be (batch, n_in / 8)")
-        return _viterbi_decode_packed(coded, trellis, tb_depth, out)
+    hard = decoding_type == "hard"
+    two_d = getattr(coded, "ndim", None) == 2 or (hasattr(coded, "dim") and coded.dim() == 2)
+    if packed and not hard:
+        raise ValueError("packed=True is a hard-decision format")
+    if packed and not two_d:
+        raise ValueError("coded must be (batch, n_in / 8)")
     torch = _lib.require_cuda()
     lib = _lib.load()
-    hard = decoding_type == "hard"
-    if getattr(coded, "ndim", None) != 2 and not (hasattr(coded, "dim") and coded.dim() == 2):
+    if not two_d:
         raise ValueError("coded must be (batch, n_in)")
-    on_device = hasattr(coded, "data_ptr") and coded.is_cuda
+    is_torch = hasattr(coded, "data_ptr")
+    on_device = is_torch and coded.is_cuda
     handle = _trellis_handle(trellis)
-    if on_device:
-        x = coded
+    if packed:
+        x = coded.contiguous() if is_torch else np.ascontiguousarray(coded)
+        if x.dtype != (torch.uint8 if is_torch else np.uint8):
+            raise ValueError("packed input must be uint8")
+    elif is_torch:
         want = torch.uint8 if hard else torch.float32
-        if x.dtype != want:
-            x = x.to(want)
-        x = x.contiguous()
-        batch, n_in = x.shape
-        L, T = _sizes(trellis, n_in)
-        _check_depth(trellis, L, T, tb_depth)
-        if out is None:
-            out_t = torch.empty((batch, L), dtype=torch.uint8, device=x.device)
-        else:
-            _check_out(out, (batch, L), x, torch)
-            out_t = out
-        rc = lib.cpb_viterbi_decode(handle, _lib.ptr(x), _lib.CPB_U8 if hard else _lib.CPB_F32,
-                                    C.c_int64(batch), C.c_int64(n_in), int(tb_depth or 0),
-                                    _lib.VITERBI_MODES[decoding_type], _lib.ptr(out_t),
-                                    C.c_void_p(0), C.c_size_t(0), _lib.stream_ptr(torch))
-        _lib.check(rc, "viterbi_decode")
-        return out_t
-    x, batch, n_in = _host_buffer(coded, hard, torch)
-    L, T = _sizes(trellis, n_in)
-    _check_depth(trellis, L, T, tb_depth)
-    if out is None:
-        out = torch.empty((batch, L), dtype=torch.uint8) if hasattr(coded, "data_ptr") else np.empty((batch, L), np.uint8)
+        x = (coded if coded.dtype == want else coded.to(want)).contiguous()
     else:
-        _check_out(out, (batch, L), x, torch)
-    rc = lib.cpb_viterbi_decode_host(handle, _lib.ptr(x), _lib.CPB_U8 if hard else _lib.CPB_F32, C.c_int64(batch),
-                                     C.c_int64(n_in), int(tb_depth or 0), _lib.VITERBI_MODES[decoding_type],
-                                     _lib.ptr(out))
-    _lib.check(rc, "viterbi_decode")
+        x = _numpy_rows(coded, hard)
+    batch, n_in = x.shape[0], x.shape[1] * (8 if packed else 1)
+    L = _decoded_bits(trellis, n_in, tb_depth)
+    if packed and L % 8:
+        raise NotImplementedError("packed decode needs a whole number of output bytes per frame")
+    shape = (batch, L // 8 if packed else L)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.uint8, device=x.device) if is_torch else np.empty(shape, np.uint8)
+    else:
+        _check_out(out, shape, x, torch)
+    depth = int(tb_depth or 0)
+    in_dtype, mode = _lib.CPB_U8 if hard else _lib.CPB_F32, _lib.VITERBI_MODES[decoding_type]
+    if packed and on_device:
+        rc = lib.cpb_viterbi_decode_packed(handle, _lib.ptr(x), C.c_int64(batch), C.c_int64(n_in), depth, _lib.ptr(out),
+                                           _lib.stream_ptr(torch))
+    elif packed:
+        rc = lib.cpb_viterbi_decode_host_packed(handle, _lib.ptr(x), C.c_int64(batch), C.c_int64(n_in), depth, _lib.ptr(out))
+    elif on_device:
+        rc = lib.cpb_viterbi_decode(handle, _lib.ptr(x), in_dtype, C.c_int64(batch), C.c_int64(n_in), depth, mode,
+                                    _lib.ptr(out), C.c_void_p(0), C.c_size_t(0), _lib.stream_ptr(torch))
+    else:
+        rc = lib.cpb_viterbi_decode_host(handle, _lib.ptr(x), in_dtype, C.c_int64(batch), C.c_int64(n_in), depth, mode,
+                                         _lib.ptr(out))
+    _lib.check(rc, "viterbi_decode (packed)" if packed else "viterbi_decode")
     return out
 
 
@@ -396,8 +348,7 @@ def viterbi_decode_punctured_batch(llr, trellis, punct_vec, shouldbe, tb_depth=N
         raise ValueError("llr must be (batch, n_kept)")
     pv = np.ascontiguousarray(punct_vec, dtype=np.int32)
     batch, n_kept = x.shape
-    L, T = _sizes(trellis, int(shouldbe))
-    _check_depth(trellis, L, T, tb_depth)
+    L = _decoded_bits(trellis, int(shouldbe), tb_depth)
     handle = _trellis_handle(trellis)
     out = torch.empty((batch, L), dtype=torch.uint8, device=x.device)
     rc = lib.cpb_viterbi_decode_punctured(handle, _lib.ptr(x), C.c_int64(batch), C.c_int64(n_kept), _lib.ptr(pv), int(len(pv)),

@@ -801,13 +801,18 @@ __global__ void frame_scale_kernel(const float *__restrict__ x, int64_t n_in, in
     }
 }
 
-template <class CODE, int PACK, int IOP = 0>
+// The four kernel forms: hard decision on byte-per-bit or bit-packed rows, soft / unquantized on float rows, and the same
+// on punctured float rows.  The form fixes the kernel, how many frames a thread holds (PACK) and how it reads a row.
+enum Form { HARD, HARD_PACKED, SOFT, SOFT_PUNCT };
+
+template <class CODE, int FORM>
 static int launch(const Params &p, cudaStream_t st)
 {
+    constexpr int PACK = (FORM == HARD || FORM == HARD_PACKED) ? 2 : 1;
     const size_t smem = smem_bytes(p.RB, p.TBB, PACK);
-    void (*kern)(const Params) = (IOP == 1) ? viterbi_fast_kernel_hard_packed<CODE>
-                               : (IOP == 2) ? viterbi_fast_kernel_soft_punct<CODE>
-                               : (PACK == 2) ? viterbi_fast_kernel_hard<CODE> : viterbi_fast_kernel_soft<CODE>;
+    void (*kern)(const Params) = (FORM == HARD) ? viterbi_fast_kernel_hard<CODE>
+                               : (FORM == HARD_PACKED) ? viterbi_fast_kernel_hard_packed<CODE>
+                               : (FORM == SOFT) ? viterbi_fast_kernel_soft<CODE> : viterbi_fast_kernel_soft_punct<CODE>;
 #ifndef CPB_SOFT_MAX_CARVEOUT
 #define CPB_SOFT_MAX_CARVEOUT 0
 #endif
@@ -819,6 +824,25 @@ static int launch(const Params &p, cudaStream_t st)
 }
 
 }  // namespace fast
+
+// The codes with register-resident kernels.  A trellis's fast_id is 1 + the index of its code in this list, 0 for none.
+template <class... CODES>
+struct CodeList {
+    static int fast_id(const cpbTrellis &t)
+    {
+        int id = 0, i = 0;
+        ((++i, id = (id == 0 && code_matches<CODES>(t)) ? i : id), ...);
+        return id;
+    }
+    template <int FORM>
+    static int launch(int fast_id, const fast::Params &p, cudaStream_t st)
+    {
+        int rc = CPB_EUNSUPPORTED, i = 0;
+        ((++i == fast_id ? rc = fast::launch<CODES, FORM>(p, st) : 0), ...);
+        return rc;
+    }
+};
+using FastCodes = CodeList<Code133_171, Code171_133, Code5_43, Code5_7>;
 
 // ------------------------------------------------------------------------------------------------
 // Generic table-driven path
@@ -991,10 +1015,7 @@ int cpb_trellis_create(const int32_t *next_state, const int32_t *output, int k, 
         cpb_trellis_destroy(t);
         return CPB_ECUDA;
     }
-    if (code_matches<Code133_171>(*t)) t->fast_id = 1;
-    else if (code_matches<Code171_133>(*t)) t->fast_id = 2;
-    else if (code_matches<Code5_43>(*t)) t->fast_id = 3;
-    else if (code_matches<Code5_7>(*t)) t->fast_id = 4;
+    t->fast_id = FastCodes::fast_id(*t);
     *out = t;
     return CPB_OK;
 }
@@ -1024,14 +1045,15 @@ void cpb_trellis_host_tables(const cpbTrellis *t, const int32_t **next, const in
     *out = t->output.data();
 }
 
-static int resolve_depth(const cpbTrellis *t, int64_t L, int tb_depth)
+// L, T and the traceback depth D of a decode of n_in coded values (tb_depth <= 0: the reference default min(5 M, L),
+// convcode.py:701-702).  CPB_EINVAL where the reference returns uninitialised memory -- no traceback window ever closes
+// (T < D - 1) or D < 2 -- and for more trellis steps than the kernels count.
+struct Dims { int64_t L = 0, T = 0; int D = 0; };
+static int viterbi_dims(const cpbTrellis *t, int64_t n_in, int tb_depth, Dims &d)
 {
-    if (tb_depth <= 0) {
-        int64_t d = 5 * (int64_t)t->M;          // convcode.py:701-702
-        if (d > L) d = L;
-        return (int)d;
-    }
-    return tb_depth;
+    cpb_viterbi_sizes(t, n_in, &d.L, &d.T);
+    d.D = (tb_depth > 0) ? tb_depth : (int)std::min<int64_t>(5 * (int64_t)t->M, d.L);
+    return (d.L <= 0 || d.D < 2 || d.T < d.D - 1 || d.T > (1 << 24)) ? CPB_EINVAL : CPB_OK;
 }
 
 static bool use_fast(const cpbTrellis *t, int D, int mode, int in_dtype)
@@ -1058,30 +1080,58 @@ static size_t generic_chunk(const cpbTrellis *t, int64_t batch, int64_t T, int64
     return (size_t)((T + 1) * (int64_t)(t->S + 1) * chunk);
 }
 
-static int launch_fast(const cpbTrellis *t, const fast::Params &p, int pack, int packed_io, cudaStream_t st)
+// fast form of a decode of byte-per-bit or float rows
+static int row_form(int mode) { return (mode == CPB_VITERBI_HARD) ? fast::HARD : fast::SOFT; }
+
+// scratch bytes of a fast-path decode: 256, then one scale per frame for the float forms (the packed form takes no workspace)
+static size_t fast_scratch_bytes(int form, int64_t batch)
 {
-    if (packed_io == 2) {
-        if (t->fast_id == 1) return fast::launch<Code133_171, 1, 2>(p, st);
-        if (t->fast_id == 2) return fast::launch<Code171_133, 1, 2>(p, st);
-        if (t->fast_id == 3) return fast::launch<Code5_43, 1, 2>(p, st);
-        return fast::launch<Code5_7, 1, 2>(p, st);
+    if (form == fast::HARD_PACKED) return 0;
+    return 256 + (form == fast::HARD ? 0 : (size_t)batch * sizeof(float));
+}
+
+// the fast::Params fields every form shares; CPB_EUNSUPPORTED when the kernel's shared memory does not fit
+static int fast_params(int form, const Dims &d, int mode, const void *coded, int64_t n_in, int64_t batch, uint8_t *out,
+                       fast::Params &p)
+{
+    const int pack = (form == fast::HARD || form == fast::HARD_PACKED) ? 2 : 1;
+    p = fast::Params{};
+    p.coded = coded; p.n_in = n_in; p.batch = batch;
+    p.L = (int)d.L; p.T = (int)d.T; p.D = d.D;
+    p.TBB = (pack == 2) ? CPB_VITERBI_TBB : CPB_VITERBI_TBB_SOFT;
+    p.NJ = (d.D > 8) ? (d.D - 8 + fast::B - 1) / fast::B : 0;
+    p.RB = p.NJ + p.TBB / fast::B;
+    p.mode = mode; p.out = out;
+    p.out_vec8 = ((d.L % 8) == 0 && (((uintptr_t)out) % 8) == 0) ? 1 : 0;
+    p.met_mask = (pack == 2) ? ~fast::KeyOps<2>::FMASK : ~fast::KeyOps<1>::FMASK;
+    return (fast::smem_bytes(p.RB, p.TBB, pack) > device_props().smem_optin) ? CPB_EUNSUPPORTED : CPB_OK;
+}
+
+// Acquires the form's scratch, computes the per-frame scales of the float forms from the first n_used values of each row
+// (row_len values apart), launches the kernel of the trellis's code and releases the scratch.
+static int fast_run(const cpbTrellis *t, int form, fast::Params &p, int64_t row_len, int64_t n_used, void *workspace,
+                    size_t workspace_bytes, cudaStream_t st)
+{
+    Scratch ws;
+    int rc = ws.acquire(workspace, workspace_bytes, fast_scratch_bytes(form, p.batch), st);
+    if (rc) return rc;
+    if (form == fast::SOFT || form == fast::SOFT_PUNCT) {
+        float *sc = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ws.ptr) + 256);
+        p.frame_scale = sc;
+        const int wpb = 8;
+        fast::frame_scale_kernel<<<(unsigned)ceil_div(p.batch, wpb), wpb * 32, 0, st>>>(
+            reinterpret_cast<const float *>(p.coded), row_len, n_used, p.batch, p.mode, sc);
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) { ws.release(); return record_cuda_error(e, "frame_scale_kernel", __FILE__, __LINE__); }
     }
-    if (packed_io) {
-        if (t->fast_id == 1) return fast::launch<Code133_171, 2, 1>(p, st);
-        if (t->fast_id == 2) return fast::launch<Code171_133, 2, 1>(p, st);
-        if (t->fast_id == 3) return fast::launch<Code5_43, 2, 1>(p, st);
-        return fast::launch<Code5_7, 2, 1>(p, st);
+    switch (form) {
+    case fast::HARD: rc = FastCodes::launch<fast::HARD>(t->fast_id, p, st); break;
+    case fast::HARD_PACKED: rc = FastCodes::launch<fast::HARD_PACKED>(t->fast_id, p, st); break;
+    case fast::SOFT: rc = FastCodes::launch<fast::SOFT>(t->fast_id, p, st); break;
+    default: rc = FastCodes::launch<fast::SOFT_PUNCT>(t->fast_id, p, st); break;
     }
-    if (pack == 2) {
-        if (t->fast_id == 1) return fast::launch<Code133_171, 2>(p, st);
-        if (t->fast_id == 2) return fast::launch<Code171_133, 2>(p, st);
-        if (t->fast_id == 3) return fast::launch<Code5_43, 2>(p, st);
-        return fast::launch<Code5_7, 2>(p, st);
-    }
-    if (t->fast_id == 1) return fast::launch<Code133_171, 1>(p, st);
-    if (t->fast_id == 2) return fast::launch<Code171_133, 1>(p, st);
-    if (t->fast_id == 3) return fast::launch<Code5_43, 1>(p, st);
-    return fast::launch<Code5_7, 1>(p, st);
+    ws.release();
+    return rc;
 }
 
 extern "C" {
@@ -1098,13 +1148,14 @@ int cpb_viterbi_sizes(const cpbTrellis *t, int64_t n_in, int64_t *L, int64_t *T)
 int cpb_viterbi_workspace_bytes(const cpbTrellis *t, int64_t batch, int64_t n_in, int tb_depth, int mode, size_t *bytes)
 {
     if (!t || !bytes || batch < 0) return CPB_EINVAL;
-    int64_t L, T;
-    cpb_viterbi_sizes(t, n_in, &L, &T);
-    const int D = resolve_depth(t, L, tb_depth);
-    const int in_dtype = (mode == CPB_VITERBI_HARD) ? CPB_U8 : CPB_F32;
-    if (use_fast(t, D, mode, in_dtype)) { *bytes = 256 + (mode == CPB_VITERBI_HARD ? 0 : (size_t)batch * sizeof(float)); return CPB_OK; }
+    Dims d;
+    viterbi_dims(t, n_in, tb_depth, d);          // sizes the decode rejects need no particular answer
+    if (use_fast(t, d.D, mode, mode == CPB_VITERBI_HARD ? CPB_U8 : CPB_F32)) {
+        *bytes = fast_scratch_bytes(row_form(mode), batch);
+        return CPB_OK;
+    }
     int64_t stride;
-    *bytes = generic_chunk(t, batch, T, &stride) + 256;
+    *bytes = generic_chunk(t, batch, d.T, &stride) + 256;
     return CPB_OK;
 }
 
@@ -1117,55 +1168,28 @@ int cpb_viterbi_decode(const cpbTrellis *t, const void *coded_dev, int in_dtype,
     if (!t || !coded_dev || !out_bits_dev || batch < 0 || n_in < 0) return CPB_EINVAL;
     if (in_dtype != CPB_U8 && in_dtype != CPB_F32) return CPB_EINVAL;
     if (mode != CPB_VITERBI_HARD && in_dtype != CPB_F32) return CPB_EINVAL;
-    if (batch == 0) return CPB_OK;
-    int64_t L, T;
-    cpb_viterbi_sizes(t, n_in, &L, &T);
-    const int D = resolve_depth(t, L, tb_depth);
-    // the reference returns uninitialised memory when no traceback window ever closes (T < D-1) or D < 2
-    if (L <= 0 || D < 2 || T < D - 1 || T > (1 << 24)) return CPB_EINVAL;
+    Dims d;
+    if (viterbi_dims(t, n_in, tb_depth, d)) return CPB_EINVAL;
     cudaStream_t st = (cudaStream_t)stream;
-    const DeviceProps &dp = device_props();
 
-    if (use_fast(t, D, mode, in_dtype)) {
-        fast::Params p{};
-        p.coded = coded_dev; p.n_in = n_in; p.batch = batch;
-        p.L = (int)L; p.T = (int)T; p.D = D;
-        p.TBB = (mode == CPB_VITERBI_HARD) ? CPB_VITERBI_TBB : CPB_VITERBI_TBB_SOFT;
-        p.NJ = (D > 8) ? (D - 8 + fast::B - 1) / fast::B : 0;
-        p.RB = p.NJ + p.TBB / fast::B;
-        p.mode = mode; p.out = out_bits_dev;
-        p.out_vec8 = ((L % 8) == 0 && (((uintptr_t)out_bits_dev) % 8) == 0) ? 1 : 0;
-        const int pack = (mode == CPB_VITERBI_HARD) ? 2 : 1;
-        const size_t need = 256 + (pack == 1 ? (size_t)batch * sizeof(float) : 0);
-        Scratch ws;
-        int rc = ws.acquire(workspace_dev, workspace_bytes, need, st);
+    if (use_fast(t, d.D, mode, in_dtype)) {
+        const int form = row_form(mode);
+        fast::Params p;
+        int rc = fast_params(form, d, mode, coded_dev, n_in, batch, out_bits_dev, p);
         if (rc) return rc;
-        if (fast::smem_bytes(p.RB, p.TBB, pack) > dp.smem_optin) { ws.release(); return CPB_EUNSUPPORTED; }
-        p.met_mask = (pack == 2) ? ~fast::KeyOps<2>::FMASK : ~fast::KeyOps<1>::FMASK;
-        if (pack == 2) p.in_aligned = ((n_in % 4) == 0 && (((uintptr_t)coded_dev) % 4) == 0) ? 1 : 0;
-        else p.in_aligned = ((n_in % 4) == 0 && (((uintptr_t)coded_dev) % 16) == 0) ? 1 : 0;
-        if (pack == 1) {
-            float *sc = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ws.ptr) + 256);
-            p.frame_scale = sc;
-            const int wpb = 8;
-            fast::frame_scale_kernel<<<(unsigned)ceil_div(batch, wpb), wpb * 32, 0, st>>>(
-                reinterpret_cast<const float *>(coded_dev), n_in, 2 * L, batch, mode, sc);
-            cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) { ws.release(); return record_cuda_error(e, "frame_scale_kernel", __FILE__, __LINE__); }
-        }
-        rc = launch_fast(t, p, pack, 0, st);
-        ws.release();
-        return rc;
+        p.in_aligned = ((n_in % 4) == 0 && (((uintptr_t)coded_dev) % (form == fast::HARD ? 4 : 16)) == 0) ? 1 : 0;
+        return fast_run(t, form, p, n_in, 2 * d.L, workspace_dev, workspace_bytes, st);
     }
 
     // generic path, chunked so the survivor scratch stays bounded
+    const int64_t L = d.L, T = d.T;
     int64_t stride = 0;
     const size_t need = generic_chunk(t, batch, T, &stride);
     Scratch ws;
     int rc = ws.acquire(workspace_dev, workspace_bytes, need, st);
     if (rc) return rc;
     const size_t smem = sizeof(float) * ((size_t)2 * t->S + (1u << t->n)) * gen::BD;
-    if (smem > dp.smem_optin) { ws.release(); return CPB_EUNSUPPORTED; }
+    if (smem > device_props().smem_optin) { ws.release(); return CPB_EUNSUPPORTED; }
     { const int rc_ = ensure_dyn_smem(reinterpret_cast<const void *>(gen::viterbi_generic_kernel), smem); if (rc_) { ws.release(); return rc_; } }
     cudaError_t e = cudaSuccess;
     for (int64_t f0 = 0; f0 < batch; f0 += stride) {
@@ -1174,7 +1198,7 @@ int cpb_viterbi_decode(const cpbTrellis *t, const void *coded_dev, int in_dtype,
         p.nframes = (int)std::min<int64_t>(stride, batch - f0);
         p.stride = stride; p.pred = t->pred_dev;
         p.k = t->k; p.n = t->n; p.S = t->S; p.I = t->I;
-        p.L = (int)L; p.T = (int)T; p.D = D; p.mode = mode;
+        p.L = (int)L; p.T = (int)T; p.D = d.D; p.mode = mode;
         p.winners = reinterpret_cast<uint8_t *>(ws.ptr);
         p.best = p.winners + (size_t)(T + 1) * t->S * stride;
         p.out = out_bits_dev;
@@ -1192,34 +1216,24 @@ int cpb_viterbi_decode_packed(const cpbTrellis *t, const uint8_t *coded_packed_d
 {
     if (t && batch == 0) return CPB_OK;
     if (!t || !coded_packed_dev || !out_packed_dev || batch < 0 || n_in <= 0) return CPB_EINVAL;
-    int64_t L, T;
-    cpb_viterbi_sizes(t, n_in, &L, &T);
-    const int D = resolve_depth(t, L, tb_depth);
-    if (L <= 0 || D < 2 || T < D - 1 || T > (1 << 24)) return CPB_EINVAL;
+    Dims d;
+    if (viterbi_dims(t, n_in, tb_depth, d)) return CPB_EINVAL;
     // whole bytes per row, whole output bytes per traceback block
-    if (!use_fast(t, D, CPB_VITERBI_HARD, CPB_U8) || (n_in % 8) != 0 || (L % 8) != 0 || ((D - 2) % 4) != 0 ||
+    if (!use_fast(t, d.D, CPB_VITERBI_HARD, CPB_U8) || (n_in % 8) != 0 || (d.L % 8) != 0 || ((d.D - 2) % 4) != 0 ||
         (CPB_VITERBI_TBB % 8) != 0)
         return CPB_EUNSUPPORTED;
-    const DeviceProps &dp = device_props();
-    fast::Params p{};
-    p.coded = coded_packed_dev; p.n_in = n_in; p.batch = batch;
-    p.L = (int)L; p.T = (int)T; p.D = D;
-    p.TBB = CPB_VITERBI_TBB;
-    p.NJ = (D > 8) ? (D - 8 + fast::B - 1) / fast::B : 0;
-    p.RB = p.NJ + p.TBB / fast::B;
-    p.mode = CPB_VITERBI_HARD; p.out = out_packed_dev;
+    fast::Params p;
+    const int rc = fast_params(fast::HARD_PACKED, d, CPB_VITERBI_HARD, coded_packed_dev, n_in, batch, out_packed_dev, p);
+    if (rc) return rc;
     p.out_vec8 = 2;
-    p.in_aligned = 0;
-    p.met_mask = ~fast::KeyOps<2>::FMASK;
-    if (fast::smem_bytes(p.RB, p.TBB, 2) > dp.smem_optin) return CPB_EUNSUPPORTED;
-    return launch_fast(t, p, 2, 1, (cudaStream_t)stream);
+    return fast_run(t, fast::HARD_PACKED, p, 0, 0, nullptr, 0, (cudaStream_t)stream);
 }
 
 
 int cpb_viterbi_punctured_workspace_bytes(int64_t batch, size_t *bytes)
 {
     if (!bytes || batch < 0) return CPB_EINVAL;
-    *bytes = 256 + (size_t)batch * sizeof(float);
+    *bytes = fast_scratch_bytes(fast::SOFT_PUNCT, batch);
     return CPB_OK;
 }
 
@@ -1238,37 +1252,15 @@ int cpb_viterbi_decode_punctured(const cpbTrellis *t, const float *llr_punct_dev
     // values the depuncturing consumes (convcode.py:796-799 indexes the punctured array: IndexError when it is too short)
     const int64_t need = (n_depunct / punct_len) * ones + __builtin_popcount(mask & ((1u << (n_depunct % punct_len)) - 1u));
     if (need > n_kept) return CPB_EINVAL;
-    int64_t L, T;
-    cpb_viterbi_sizes(t, n_depunct, &L, &T);
-    const int D = resolve_depth(t, L, tb_depth);
-    if (L <= 0 || D < 2 || T < D - 1 || T > (1 << 24)) return CPB_EINVAL;
-    if (!use_fast(t, D, mode, CPB_F32)) return CPB_EUNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream;
-    const DeviceProps &dp = device_props();
-    fast::Params p{};
-    p.coded = llr_punct_dev; p.n_in = n_depunct; p.batch = batch;
-    p.L = (int)L; p.T = (int)T; p.D = D;
-    p.TBB = CPB_VITERBI_TBB_SOFT;
-    p.NJ = (D > 8) ? (D - 8 + fast::B - 1) / fast::B : 0;
-    p.RB = p.NJ + p.TBB / fast::B;
-    p.mode = mode; p.out = out_bits_dev;
-    p.out_vec8 = ((L % 8) == 0 && (((uintptr_t)out_bits_dev) % 8) == 0) ? 1 : 0;
-    p.met_mask = ~fast::KeyOps<1>::FMASK;
-    p.punct_mask = mask; p.punct_len = punct_len; p.n_kept = n_kept;
-    if (fast::smem_bytes(p.RB, p.TBB, 1) > dp.smem_optin) return CPB_EUNSUPPORTED;
-    Scratch ws;
-    int rc = ws.acquire(workspace_dev, workspace_bytes, 256 + (size_t)batch * sizeof(float), st);
+    Dims d;
+    if (viterbi_dims(t, n_depunct, tb_depth, d)) return CPB_EINVAL;
+    if (!use_fast(t, d.D, mode, CPB_F32)) return CPB_EUNSUPPORTED;
+    fast::Params p;
+    const int rc = fast_params(fast::SOFT_PUNCT, d, mode, llr_punct_dev, n_depunct, batch, out_bits_dev, p);
     if (rc) return rc;
-    float *sc = reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(ws.ptr) + 256);
-    p.frame_scale = sc;
-    const int wpb = 8;
+    p.punct_mask = mask; p.punct_len = punct_len; p.n_kept = n_kept;
     // the erasures are zeros: the frame's scale is the largest magnitude among the values the depuncturing uses
-    fast::frame_scale_kernel<<<(unsigned)ceil_div(batch, wpb), wpb * 32, 0, st>>>(llr_punct_dev, n_kept, need, batch, mode, sc);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) { ws.release(); return record_cuda_error(e, "frame_scale_kernel", __FILE__, __LINE__); }
-    rc = launch_fast(t, p, 1, 2, st);
-    ws.release();
-    return rc;
+    return fast_run(t, fast::SOFT_PUNCT, p, n_kept, need, workspace_dev, workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -151,13 +151,24 @@ def normalize_kernel_name(name):
 def launched_kernels(fn):
     """Run fn() under torch.profiler (CUDA activity only: CUPTI sees every kernel of the process, including the ones the
     ctypes library launches on its own pipeline streams) and return the normalised names of what it recorded: the
-    kernels launched, plus the runtime API calls (cudaLaunchKernel, ...) that made them."""
+    kernels launched, plus the runtime API calls (cudaLaunchKernel, ...) that made them.
+
+    Kineto maps CUPTI's GPU timestamps onto the host clock from a sync taken when CUPTI starts, and drops every GPU record
+    whose mapped time falls outside the profiling window.  On some hosts that mapping drifts by more than a second within
+    a minute of the first session, and the kernel records are then lost ("Out-of-range" in Kineto's record counts).
+    TEARDOWN_CUPTI=1 finalises CUPTI after each session, so that every session starts it, and its clock sync, afresh.
+    The teardown runs on a thread of its own and a session started before it ends records nothing: hence the pause."""
+    import os
+    import time
+
     import torch
     from torch.profiler import ProfilerActivity, profile
+    os.environ["TEARDOWN_CUPTI"] = "1"
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         fn()
         torch.cuda.synchronize()
+    time.sleep(0.1)
     names = {e.name for e in prof.events()}
     raw = getattr(prof.profiler, "kineto_results", None)                     # the raw activity records, when exposed
     if raw is not None:
