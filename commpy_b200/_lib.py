@@ -28,6 +28,7 @@ SYMBOLS = [
     "cpb_modem_create", "cpb_modem_destroy", "cpb_modem_is_separable", "cpb_demod_soft", "cpb_demod_hard",
     "cpb_demod_soft_csi", "cpb_demod_hard_csi",
     "cpb_count_errors", "cpb_conv_link_tx", "cpb_conv_link_tx_punctured", "cpb_conv_link_tx_fading", "cpb_turbo_link_tx",
+    "cpb_turbo_link_tx_fading", "cpb_bpsk_combine",
 ]
 
 _lib = None

@@ -11,6 +11,19 @@
 // Randomness is counter based (Philox4x32-10, same keying as txlink.cu): message bit i of global frame f is bit (i & 127)
 // of Philox(counter = (f_lo, f_hi, i >> 7, 0), key = seed); the noise of values 4q .. 4q+3 of stream j comes from
 // Philox(counter = (f_lo, f_hi, q, 2 + j), key = seed) through Box-Muller.  Nothing depends on the batch split.
+//
+// Flat fading (FADING = true, cpb_turbo_link_tx_fading; SISOFlatChannel, commpy/channels.py:176-221): value t of stream j
+// (0 = sys, 1 = par1, 2 = par2), q = t >> 2, is received as y = h x + sigma (n_re + j n_im), x = 2 bit - 1, with
+//     n_re  the noise above: Philox(f_lo, f_hi, q, 2 + j), values 4q .. 4q+3
+//     n_im  Philox(f_lo, f_hi, q, 5 + j) through the same Box-Muller, values 4q .. 4q+3 in the same order
+//     h     mean + sqrt(nlos / 2) (g.x + j g.y); values 4q, 4q+1 from Philox(f_lo, f_hi, 2q, 8 + j), 4q+2, 4q+3 from
+//           Philox(f_lo, f_hi, 2q + 1, 8 + j): each call gives two Box-Mullers, i.e. two complex gains
+// Counter words: 0 message, 2..4 real noise, 5..7 imaginary noise, 8..10 gains.  y_re = fmaf(sigma, n_re, h_re x), so the
+// message and Re(y) at h = 1 + 0j are the AWGN link's bit for bit.
+//
+// Receiver (cpb_bpsk_combine): s = Re(conj(h) y) = |h|^2 x + N(0, sigma^2 |h|^2), whose exact LLR 2 s / sigma^2 is the
+// channel term the MAP / turbo kernels form from a symbol s at noise variance sigma^2: the decoder takes s unchanged.
+#include <cmath>
 #include <vector>
 
 #include "common.cuh"
@@ -55,7 +68,29 @@ struct Params {
     int S;
     uint8_t *msg;
     float *ysys, *ypar1, *ypar2;
+    float2 *y, *h;            // fading: [3][frames][N] complex64, stream-major
+    float mean_re, mean_im;   // fading: mean gain and per-component std of its scattered part
+    float nlos_std;
 };
+
+// fading gain of one value from two standard normals
+__device__ __forceinline__ float2 fading_gain(const Params &p, float2 g)
+{
+    return make_float2(fmaf(p.nlos_std, g.x, p.mean_re), fmaf(p.nlos_std, g.y, p.mean_im));
+}
+
+// imaginary noise (counter word 5 + j) and gains (8 + j) of values 4q .. 4q+3 of stream j
+__device__ __forceinline__ void fading_draws(const Params &p, uint32_t f_lo, uint32_t f_hi, uint32_t q, uint32_t j, float ni[4],
+                                             float2 hh[4])
+{
+    const uint4 r = philox4x32_10(make_uint4(f_lo, f_hi, q, 5u + j), p.seed_lo, p.seed_hi);
+    const float2 a = box_muller(r.x, r.y), b = box_muller(r.z, r.w);
+    ni[0] = a.x; ni[1] = a.y; ni[2] = b.x; ni[3] = b.y;
+    const uint4 g0 = philox4x32_10(make_uint4(f_lo, f_hi, 2u * q, 8u + j), p.seed_lo, p.seed_hi);
+    const uint4 g1 = philox4x32_10(make_uint4(f_lo, f_hi, 2u * q + 1u, 8u + j), p.seed_lo, p.seed_hi);
+    hh[0] = fading_gain(p, box_muller(g0.x, g0.y)); hh[1] = fading_gain(p, box_muller(g0.z, g0.w));
+    hh[2] = fading_gain(p, box_muller(g1.x, g1.y)); hh[3] = fading_gain(p, box_muller(g1.z, g1.w));
+}
 
 // message bits: one thread per 128 bits
 __global__ void __launch_bounds__(256) msg_kernel(const Params p)
@@ -73,7 +108,8 @@ __global__ void __launch_bounds__(256) msg_kernel(const Params p)
 }
 
 // one thread per (frame, component encoder): encoder 0 walks msg in natural order (and emits the systematic stream),
-// encoder 1 walks msg[p_array]
+// encoder 1 walks msg[p_array].  FADING: complex outputs y and gains h instead of the real streams.
+template <bool FADING>
 __global__ void __launch_bounds__(128) encode_kernel(const Params p)
 {
     const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -83,8 +119,13 @@ __global__ void __launch_bounds__(128) encode_kernel(const Params p)
     const uint64_t fg = (uint64_t)(p.first_frame + fl);
     const uint32_t f_lo = (uint32_t)fg, f_hi = (uint32_t)(fg >> 32);
     const uint8_t *m = p.msg + fl * p.N;
-    float *ypar = (enc ? p.ypar2 : p.ypar1) + fl * p.N;
-    float *ysys = p.ysys + fl * p.N;
+    float *ypar = FADING ? nullptr : (enc ? p.ypar2 : p.ypar1) + fl * p.N;
+    float *ysys = FADING ? nullptr : p.ysys + fl * p.N;
+    const int64_t plane = p.frames * p.N;                // fading: one stream of y / h
+    float2 *cpar = FADING ? p.y + (1 + enc) * plane + fl * p.N : nullptr;
+    float2 *hpar = FADING ? p.h + (1 + enc) * plane + fl * p.N : nullptr;
+    float2 *csys = FADING ? p.y + fl * p.N : nullptr;
+    float2 *hsys = FADING ? p.h + fl * p.N : nullptr;
     int state = 0;                                       // the encoder starts in state 0 (convcode.py:529)
     for (int64_t q = 0; q < p.N; q += 4) {
         const uint4 rp = philox4x32_10(make_uint4(f_lo, f_hi, (uint32_t)(q >> 2), 3u + (uint32_t)enc), p.seed_lo, p.seed_hi);
@@ -96,6 +137,12 @@ __global__ void __launch_bounds__(128) encode_kernel(const Params p)
             const float2 c = box_muller(rs.x, rs.y), d = box_muller(rs.z, rs.w);
             ns[0] = c.x; ns[1] = c.y; ns[2] = d.x; ns[3] = d.y;
         }
+        float nzi[4], nsi[4];
+        float2 hp[4], hs[4];
+        if (FADING) {
+            fading_draws(p, f_lo, f_hi, (uint32_t)(q >> 2), 1u + (uint32_t)enc, nzi, hp);
+            if (enc == 0) fading_draws(p, f_lo, f_hi, (uint32_t)(q >> 2), 0u, nsi, hs);
+        }
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const int64_t t = q + i;
@@ -104,21 +151,63 @@ __global__ void __launch_bounds__(128) encode_kernel(const Params p)
             const int e = 2 * state + u;
             const int par = p.par_tab[e];
             state = p.next_tab[e];
-            ypar[t] = fmaf(p.sigma, nz[i], par ? 1.0f : -1.0f);
-            if (enc == 0) ysys[t] = fmaf(p.sigma, ns[i], u ? 1.0f : -1.0f);
+            if (FADING) {
+                const float xp = par ? 1.0f : -1.0f, xs = u ? 1.0f : -1.0f;
+                cpar[t] = make_float2(fmaf(p.sigma, nz[i], hp[i].x * xp), fmaf(p.sigma, nzi[i], hp[i].y * xp));
+                hpar[t] = hp[i];
+                if (enc == 0) {
+                    csys[t] = make_float2(fmaf(p.sigma, ns[i], hs[i].x * xs), fmaf(p.sigma, nsi[i], hs[i].y * xs));
+                    hsys[t] = hs[i];
+                }
+            } else {
+                ypar[t] = fmaf(p.sigma, nz[i], par ? 1.0f : -1.0f);
+                if (enc == 0) ysys[t] = fmaf(p.sigma, ns[i], u ? 1.0f : -1.0f);
+            }
         }
+    }
+}
+
+// coherent BPSK combining: s = Re(conj(h) y) = h_re y_re + h_im y_im.  vec: y and h 16-byte aligned, s 16-byte aligned --
+// threads [0, n/4) take four values each (two 16-byte loads of y and of h, one 16-byte store), the next n % 4 threads one.
+__device__ __forceinline__ float combine1(float2 y, float2 h) { return fmaf(h.y, y.y, h.x * y.x); }
+
+__global__ void __launch_bounds__(256) bpsk_combine_kernel(const float2 *__restrict__ y, const float2 *__restrict__ h, int64_t n,
+                                                           float *__restrict__ s, int vec)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (vec) {
+        const int64_t n4 = n >> 2;
+        if (i < n4) {
+            const float4 y0 = reinterpret_cast<const float4 *>(y)[2 * i], y1 = reinterpret_cast<const float4 *>(y)[2 * i + 1];
+            const float4 h0 = reinterpret_cast<const float4 *>(h)[2 * i], h1 = reinterpret_cast<const float4 *>(h)[2 * i + 1];
+            reinterpret_cast<float4 *>(s)[i] = make_float4(combine1(make_float2(y0.x, y0.y), make_float2(h0.x, h0.y)),
+                                                           combine1(make_float2(y0.z, y0.w), make_float2(h0.z, h0.w)),
+                                                           combine1(make_float2(y1.x, y1.y), make_float2(h1.x, h1.y)),
+                                                           combine1(make_float2(y1.z, y1.w), make_float2(h1.z, h1.w)));
+            return;
+        }
+        const int64_t t = 4 * n4 + (i - n4);             // scalar tail
+        if (t < n) s[t] = combine1(y[t], h[t]);
+    } else if (i < n) {
+        s[i] = combine1(y[i], h[i]);
     }
 }
 
 }  // namespace turbolink
 
-extern "C" int cpb_turbo_link_tx(const cpbTrellis *t, const int32_t *perm_dev, int64_t frames, int64_t N, uint64_t seed,
-                                 int64_t first_frame, float noise_sigma, uint8_t *msg_dev, float *sys_dev, float *par1_dev,
-                                 float *par2_dev, void *stream)
+// fading == false: AWGN into sys / par1 / par2; otherwise flat fading into y / h ([3][frames][N] complex64)
+static int turbo_link_tx_impl(const cpbTrellis *t, const int32_t *perm_dev, int64_t frames, int64_t N, uint64_t seed,
+                              int64_t first_frame, float noise_sigma, bool fading, float mean_re, float mean_im, float nlos,
+                              uint8_t *msg_dev, float *sys_dev, float *par1_dev, float *par2_dev, float *y_dev, float *h_dev,
+                              void *stream)
 {
     if (!t || frames < 0 || N < 1 || first_frame < 0) return CPB_EINVAL;
+    if (fading && !(nlos >= 0.0f && std::isfinite(nlos) && std::isfinite(mean_re) && std::isfinite(mean_im) &&
+                    std::isfinite(noise_sigma)))
+        return CPB_EINVAL;
     if (frames == 0) return CPB_OK;
-    if (!perm_dev || !msg_dev || !sys_dev || !par1_dev || !par2_dev) return CPB_EINVAL;
+    if (!perm_dev || !msg_dev) return CPB_EINVAL;
+    if (fading ? (!y_dev || !h_dev) : (!sys_dev || !par1_dev || !par2_dev)) return CPB_EINVAL;
     int k, n, S;
     cpb_trellis_dims(t, &k, &n, &S);
     if (k != 1 || n != 2 || S > 32) return CPB_EUNSUPPORTED;
@@ -137,10 +226,44 @@ extern "C" int cpb_turbo_link_tx(const cpbTrellis *t, const int32_t *perm_dev, i
     p.seed_lo = (uint32_t)seed; p.seed_hi = (uint32_t)(seed >> 32);
     p.sigma = noise_sigma; p.perm = perm_dev;
     p.msg = msg_dev; p.ysys = sys_dev; p.ypar1 = par1_dev; p.ypar2 = par2_dev;
+    p.y = reinterpret_cast<float2 *>(y_dev); p.h = reinterpret_cast<float2 *>(h_dev);
+    p.mean_re = mean_re; p.mean_im = mean_im;
+    p.nlos_std = (float)std::sqrt(0.5 * (double)nlos);
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t blocks = (N + 127) >> 7;
     turbolink::msg_kernel<<<(unsigned)ceil_div(frames * blocks, 256), 256, 0, st>>>(p);
-    turbolink::encode_kernel<<<(unsigned)ceil_div(2 * frames, 128), 128, 0, st>>>(p);
+    if (fading) turbolink::encode_kernel<true><<<(unsigned)ceil_div(2 * frames, 128), 128, 0, st>>>(p);
+    else turbolink::encode_kernel<false><<<(unsigned)ceil_div(2 * frames, 128), 128, 0, st>>>(p);
+    CPB_LAUNCH_CHECK();
+    return CPB_OK;
+}
+
+extern "C" int cpb_turbo_link_tx(const cpbTrellis *t, const int32_t *perm_dev, int64_t frames, int64_t N, uint64_t seed,
+                                 int64_t first_frame, float noise_sigma, uint8_t *msg_dev, float *sys_dev, float *par1_dev,
+                                 float *par2_dev, void *stream)
+{
+    return turbo_link_tx_impl(t, perm_dev, frames, N, seed, first_frame, noise_sigma, false, 0.0f, 0.0f, 0.0f, msg_dev, sys_dev,
+                              par1_dev, par2_dev, nullptr, nullptr, stream);
+}
+
+extern "C" int cpb_turbo_link_tx_fading(const cpbTrellis *t, const int32_t *perm_dev, int64_t frames, int64_t N, uint64_t seed,
+                                        int64_t first_frame, float noise_sigma, float mean_re, float mean_im, float nlos,
+                                        uint8_t *msg_dev, float *y_dev, float *h_dev, void *stream)
+{
+    return turbo_link_tx_impl(t, perm_dev, frames, N, seed, first_frame, noise_sigma, true, mean_re, mean_im, nlos, msg_dev,
+                              nullptr, nullptr, nullptr, y_dev, h_dev, stream);
+}
+
+extern "C" int cpb_bpsk_combine(const float *y_dev, const float *h_dev, int64_t n, float *s_dev, void *stream)
+{
+    if (n < 0) return CPB_EINVAL;
+    if (n == 0) return CPB_OK;
+    if (!y_dev || !h_dev || !s_dev) return CPB_EINVAL;
+    const bool vec = ((reinterpret_cast<uintptr_t>(y_dev) | reinterpret_cast<uintptr_t>(h_dev) |
+                       reinterpret_cast<uintptr_t>(s_dev)) & 15) == 0;
+    const int64_t threads = vec ? (n >> 2) + (n & 3) : n;
+    turbolink::bpsk_combine_kernel<<<(unsigned)ceil_div(threads, 256), 256, 0, (cudaStream_t)stream>>>(
+        reinterpret_cast<const float2 *>(y_dev), reinterpret_cast<const float2 *>(h_dev), n, s_dev, vec ? 1 : 0);
     CPB_LAUNCH_CHECK();
     return CPB_OK;
 }

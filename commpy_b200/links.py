@@ -13,6 +13,10 @@
   stop decision (`links.py:313`).  With `fading_param` the batched link runs over SISO flat fading instead
   (`conv_link_tx_fading` -> cpb_conv_link_tx_fading, one gain per symbol as `channels.SISOFlatChannel` draws them), and
   the demapper uses the gains (cpb_demod_soft_csi / cpb_demod_hard_csi).
+* `TurboLinkGPU` is the batched rate-1/3 turbo link over BPSK (`turbo_link_tx` -> cpb_turbo_link_tx, the turbo decoder,
+  the error counter).  With `fading_param` it runs over SISO flat fading (`turbo_link_tx_fading` ->
+  cpb_turbo_link_tx_fading, one gain per coded bit), and the receiver combines coherently (`bpsk_combine` ->
+  cpb_bpsk_combine, s = Re(conj(h) y)) before the unchanged turbo decoder.
 """
 import math
 from fractions import Fraction
@@ -23,7 +27,7 @@ import numpy as np
 from . import _lib, parallel
 
 __all__ = ["link_performance", "LinkModel", "AwgnSisoChannel", "ConvLinkGPU", "conv_link_tx", "conv_link_tx_fading",
-           "idd_decoder"]
+           "turbo_link_tx_fading", "bpsk_combine", "idd_decoder"]
 
 
 class AwgnSisoChannel:
@@ -473,26 +477,91 @@ def turbo_link_tx(trellis, interleaver, frames, frame_bits, seed, first_frame, n
     return msg, ys, y1, y2
 
 
+def turbo_link_tx_fading(trellis, interleaver, frames, frame_bits, seed, first_frame, noise_sigma, fading_param):
+    """`turbo_link_tx` over SISO flat fading (SISOFlatChannel, channels.py:176-221): each coded bit x = 2b - 1 of each stream
+    is received as y = h x + noise_sigma * (N(0,1) + jN(0,1)) with its own gain h = fading_param[0] + sqrt(fading_param[1] /
+    2) * (N(0,1) + jN(0,1)), e.g. (0j, 1) for Rayleigh and (m, 1 - |m|^2) for Rician fading.  The message and Re of the
+    noise are the streams of `turbo_link_tx` (at fading_param = (1 + 0j, 0), Re(y) equals its output bit for bit).
+
+    Returns (msg uint8 (frames, frame_bits), y complex64 (3, frames, frame_bits), h complex64 (3, frames, frame_bits)) as
+    CUDA tensors; stream 0 is systematic, 1 and 2 the parity streams.  `bpsk_combine(y, h)` gives what turbo_decode
+    takes at noise_variance = noise_sigma ** 2."""
+    import ctypes as C
+    from .channelcoding.convcode import _trellis_handle
+    from .channelcoding.turbo import _checked_perm
+    mean, nlos = _fading(fading_param)
+    torch = _lib.require_cuda()
+    N = int(frame_bits)
+    perm = torch.from_numpy(_checked_perm(interleaver, N)).cuda()
+    msg = torch.empty((int(frames), N), dtype=torch.uint8, device="cuda")
+    y, h = (torch.empty((3, int(frames), N), dtype=torch.complex64, device="cuda") for _ in range(2))
+    rc = _lib.load().cpb_turbo_link_tx_fading(_trellis_handle(trellis), _lib.ptr(perm), C.c_int64(int(frames)), C.c_int64(N),
+                                              C.c_uint64(int(seed) & ((1 << 64) - 1)), C.c_int64(int(first_frame)),
+                                              C.c_float(float(noise_sigma)), C.c_float(mean.real), C.c_float(mean.imag),
+                                              C.c_float(nlos), _lib.ptr(msg), _lib.ptr(y), _lib.ptr(h), _lib.stream_ptr(torch))
+    _lib.check(rc, "turbo_link_tx_fading")
+    return msg, y, h
+
+
+def bpsk_combine(y, h):
+    """Coherent BPSK combining (cpb_bpsk_combine): s = Re(conj(h) y) for complex64 CUDA tensors y and h of one shape;
+    returns float32 s of that shape.  For y = h x + sigma (n_re + j n_im), s = |h|^2 x + N(0, sigma^2 |h|^2), whose exact
+    LLR 2 s / sigma^2 is what map_decode / turbo_decode compute from s at noise_variance = sigma^2."""
+    import ctypes as C
+    torch = _lib.require_cuda()
+    for name, t in (("y", y), ("h", h)):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.complex64:
+            raise ValueError("bpsk_combine: %s must be a complex64 CUDA tensor" % name)
+    if y.shape != h.shape:
+        raise ValueError("bpsk_combine: y and h must have the same shape, got %s and %s" % (tuple(y.shape), tuple(h.shape)))
+    y, h = y.contiguous(), h.contiguous()
+    s = torch.empty(y.shape, dtype=torch.float32, device=y.device)
+    rc = _lib.load().cpb_bpsk_combine(_lib.ptr(y), _lib.ptr(h), C.c_int64(y.numel()), _lib.ptr(s), _lib.stream_ptr(torch))
+    _lib.check(rc, "bpsk_combine")
+    return s
+
+
 class TurboLinkGPU:
     """Batched rate-1/3 turbo link over BPSK-AWGN on the GPU(s): frames generated (cpb_turbo_link_tx), decoded
-    (cpb_turbo_decode) and counted (cpb_count_errors) on the device; the error counters are the only thing all-reduced."""
+    (cpb_turbo_decode) and counted (cpb_count_errors) on the device; the error counters are the only thing all-reduced.
 
-    def __init__(self, trellis, interleaver, frame_bits, frames_per_batch=1024, iterations=6, seed=0):
+    `fading_param` (a SISOFlatChannel fading_param with a complex mean, e.g. (0j, 1) for Rayleigh): the link runs over i.i.d.
+    flat fading, one gain per coded bit (cpb_turbo_link_tx_fading), and the receiver, which knows the gains, combines each
+    value coherently (cpb_bpsk_combine) before the same turbo decoder at the same noise variance; None: AWGN."""
+
+    def __init__(self, trellis, interleaver, frame_bits, frames_per_batch=1024, iterations=6, seed=0, fading_param=None):
+        self.fading_param = fading_param
+        if fading_param is not None:
+            _fading(fading_param)
         self.trellis, self.interleaver = trellis, interleaver
         self.frame_bits, self.frames, self.iterations, self.seed = int(frame_bits), int(frames_per_batch), int(iterations), int(seed)
 
     def noise_variance(self, ebn0_db):
+        """sigma^2 per real component at Eb/N0 (dB) for rate 1/3 and Es = 1; over fading E|h|^2 = 1 for every valid
+        fading_param, so Eb/N0 is the mean Eb/N0."""
         return 1.0 / (2.0 * (1.0 / 3.0) * 10 ** (ebn0_db / 10.0))
 
     def make_batch(self, ebn0_db, batch_index):
+        """(msg, sys, par1, par2, sigma^2) over AWGN; (msg, y, h, sigma^2) over fading (y, h: (3, frames, frame_bits))."""
         rank, world, _ = parallel.world()
         first = parallel.batch_first_frame(batch_index, self.frames, rank, max(world, 1))
         s2 = self.noise_variance(ebn0_db)
+        if self.fading_param is not None:
+            return turbo_link_tx_fading(self.trellis, self.interleaver, self.frames, self.frame_bits, self.seed, first,
+                                        math.sqrt(s2), self.fading_param) + (s2,)
         return turbo_link_tx(self.trellis, self.interleaver, self.frames, self.frame_bits, self.seed, first, math.sqrt(s2)) + (s2,)
 
-    def decode_count(self, msg, ys, y1, y2, s2, counters, torch):
+    def decode_count(self, msg, *args):
+        """decode_count(*make_batch(...), counters, torch): decode(msg, sys, par1, par2, s2, counters, torch) over AWGN,
+        (msg, y, h, s2, counters, torch) over fading -- y and h are combined first.  Adds the errors to `counters`."""
         import ctypes as C
         from .channelcoding import turbo_decode_batch
+        *rx, s2, counters, torch = args
+        if self.fading_param is not None:
+            y, h = rx
+            ys, y1, y2 = bpsk_combine(y, h)
+        else:
+            ys, y1, y2 = rx
         dec = turbo_decode_batch(ys, y1, y2, self.trellis, s2, self.iterations, self.interleaver)
         L = msg.shape[1]
         rc = _lib.load().cpb_count_errors(_lib.ptr(dec), _lib.ptr(msg), C.c_int64(msg.shape[0]), C.c_int64(L), C.c_int64(L),
@@ -508,11 +577,11 @@ class TurboLinkGPU:
         for i, e in enumerate(EbN0s):
             tot = torch.zeros(3, dtype=torch.int64, device="cuda")
             while True:
-                msg, ys, y1, y2, s2 = self.make_batch(float(e), batch_index)
+                batch = self.make_batch(float(e), batch_index)
                 batch_index += 1
                 local = torch.zeros(3, dtype=torch.int64, device="cuda")
-                self.decode_count(msg, ys, y1, y2, s2, local, torch)
-                local[2] = msg.numel()
+                self.decode_count(*batch, local, torch)
+                local[2] = batch[0].numel()
                 parallel.allreduce_counters(local)
                 tot += local
                 c = tot.cpu().numpy()

@@ -250,6 +250,20 @@ int cpb_conv_link_tx_fading(const cpbTrellis *t, const cpbModem *m, int64_t fram
 int cpb_turbo_link_tx(const cpbTrellis *t, const int32_t *perm_dev, int64_t frames, int64_t N, uint64_t seed,
                       int64_t first_frame, float noise_sigma, uint8_t *msg_dev, float *sys_dev, float *par1_dev,
                       float *par2_dev, void *stream);
+/* The same over SISO flat fading (SISOFlatChannel, channels.py:176-221), receiver CSI included: value t of stream j
+ * (0 = sys, 1 = par1, 2 = par2) is received as y = h x + noise_sigma (N(0,1) + j N(0,1)), x = 2 bit - 1, with its own gain
+ * h = (mean_re + j mean_im) + sqrt(nlos / 2) (N(0,1) + j N(0,1)).  Re of the noise is cpb_turbo_link_tx's noise; the
+ * imaginary noise and the gains come from Philox counter words 5 + j and 8 + j.  y_dev, h_dev: [3][frames][N] complex64
+ * (stream-major: stream j is a contiguous frames x N block).  With mean = 1, nlos = 0 the message and Re(y) equal
+ * cpb_turbo_link_tx's outputs bit for bit and h = 1.  CPB_EINVAL also for nlos < 0 or non-finite parameters. */
+int cpb_turbo_link_tx_fading(const cpbTrellis *t, const int32_t *perm_dev, int64_t frames, int64_t N, uint64_t seed,
+                             int64_t first_frame, float noise_sigma, float mean_re, float mean_im, float nlos,
+                             uint8_t *msg_dev, float *y_dev, float *h_dev, void *stream);
+/* Coherent BPSK combining: s[i] = Re(conj(h[i]) y[i]) = h_re y_re + h_im y_im (one fused multiply-add after one product),
+ * y_dev, h_dev: n complex64, s_dev: n float32.  s is |h|^2 x + N(0, sigma^2 |h|^2) for y = h x + sigma (n_re + j n_im), so
+ * cpb_map_decode / cpb_turbo_decode take s with noise_variance = sigma^2 and decode exactly.  s = Re(y) where h = 1 + 0j,
+ * 0 where h = 0. */
+int cpb_bpsk_combine(const float *y_dev, const float *h_dev, int64_t n, float *s_dev, void *stream);
 
 #ifdef __cplusplus
 }

@@ -70,5 +70,11 @@ link.link_performance([12.0], send_max=30000, err_min=10 ** 9)
 link = ConvLinkGPU(helpers.k7_wifi_quirk(), QAMModem(16), frame_bits=600, frames_per_batch=64, decoding_type="soft", seed=1,
                    puncture=pv, fading_param=(0.6 + 0j, 0.64))
 link.link_performance([20.0], send_max=100000, err_min=10 ** 9)
+# turbo link over fading: fading turbo TX (N not a multiple of 4), combiner (vector path + tail, unaligned scalar path)
+from commpy_b200.links import TurboLinkGPU, bpsk_combine
+link = TurboLinkGPU(rsc, RandInterlv(301, 3), 301, frames_per_batch=37, iterations=2, seed=1, fading_param=(0j, 1))
+link.link_performance([2.0], send_max=30000, err_min=10 ** 9)
+bpsk_combine(y[:4999], h[:4999])
+bpsk_combine(y[1:], h[:4999])
 torch.cuda.synchronize()
 print("sanitize driver ok")
