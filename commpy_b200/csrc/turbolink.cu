@@ -8,18 +8,13 @@
 // back to state 0, and the tails are cut off again: the three streams are those of an unterminated encoder started in
 // state 0 -- exactly what map_decode assumes (beta_N = 1 for every state, turbo.py:225-226).
 //
-// Randomness is counter based (Philox4x32-10, same keying as txlink.cu): message bit i of global frame f is bit (i & 127)
-// of Philox(counter = (f_lo, f_hi, i >> 7, 0), key = seed); the noise of values 4q .. 4q+3 of stream j comes from
-// Philox(counter = (f_lo, f_hi, q, 2 + j), key = seed) through Box-Muller.  Nothing depends on the batch split.
+// Randomness is counter based (Philox4x32-10, same keying as txlink.cu), so nothing depends on the batch split: the
+// message, noise and gain streams are the counter words of philox.cuh.
 //
-// Flat fading (FADING = true, cpb_turbo_link_tx_fading; SISOFlatChannel, commpy/channels.py:176-221): value t of stream j
-// (0 = sys, 1 = par1, 2 = par2), q = t >> 2, is received as y = h x + sigma (n_re + j n_im), x = 2 bit - 1, with
-//     n_re  the noise above: Philox(f_lo, f_hi, q, 2 + j), values 4q .. 4q+3
-//     n_im  Philox(f_lo, f_hi, q, 5 + j) through the same Box-Muller, values 4q .. 4q+3 in the same order
-//     h     mean + sqrt(nlos / 2) (g.x + j g.y); values 4q, 4q+1 from Philox(f_lo, f_hi, 2q, 8 + j), 4q+2, 4q+3 from
-//           Philox(f_lo, f_hi, 2q + 1, 8 + j): each call gives two Box-Mullers, i.e. two complex gains
-// Counter words: 0 message, 2..4 real noise, 5..7 imaginary noise, 8..10 gains.  y_re = fmaf(sigma, n_re, h_re x), so the
-// message and Re(y) at h = 1 + 0j are the AWGN link's bit for bit.
+// Flat fading (FADING = true, cpb_turbo_link_tx_fading; SISOFlatChannel, commpy/channels.py:176-221): each value
+// x = 2 bit - 1 of each stream is received as y = h x + sigma (n_re + j n_im), n_re the AWGN link's noise and
+// h = mean + sqrt(nlos / 2) (g.x + j g.y).  y_re = fmaf(sigma, n_re, h_re x), so the message and Re(y) at h = 1 + 0j are
+// the AWGN link's bit for bit.
 //
 // Receiver (cpb_bpsk_combine): s = Re(conj(h) y) = |h|^2 x + N(0, sigma^2 |h|^2), whose exact LLR 2 s / sigma^2 is the
 // channel term the MAP / turbo kernels form from a symbol s at noise variance sigma^2: the decoder takes s unchanged.
@@ -27,6 +22,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "philox.cuh"
 
 using namespace cpb;
 
@@ -35,28 +31,6 @@ void cpb_trellis_dims(const cpbTrellis *t, int *k, int *n, int *S);
 void cpb_trellis_host_tables(const cpbTrellis *t, const int32_t **next, const int32_t **out);
 
 namespace turbolink {
-
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1)
-{
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    return c;
-}
-
-__device__ __forceinline__ float2 box_muller(uint32_t a, uint32_t b)
-{
-    const float u1 = fmaf((float)a, 2.3283064365386963e-10f, 1.1641532182693481e-10f);
-    const float u2 = (float)b * 2.3283064365386963e-10f;
-    const float r = sqrtf(-2.0f * __logf(u1));
-    float sn, cs;
-    __sincosf(6.283185307179586f * u2, &sn, &cs);
-    return make_float2(r * cs, r * sn);
-}
 
 struct Params {
     int64_t frames, N, first_frame;
@@ -73,12 +47,6 @@ struct Params {
     float nlos_std;
 };
 
-// fading gain of one value from two standard normals
-__device__ __forceinline__ float2 fading_gain(const Params &p, float2 g)
-{
-    return make_float2(fmaf(p.nlos_std, g.x, p.mean_re), fmaf(p.nlos_std, g.y, p.mean_im));
-}
-
 // imaginary noise (counter word 5 + j) and gains (8 + j) of values 4q .. 4q+3 of stream j
 __device__ __forceinline__ void fading_draws(const Params &p, uint32_t f_lo, uint32_t f_hi, uint32_t q, uint32_t j, float ni[4],
                                              float2 hh[4])
@@ -88,8 +56,10 @@ __device__ __forceinline__ void fading_draws(const Params &p, uint32_t f_lo, uin
     ni[0] = a.x; ni[1] = a.y; ni[2] = b.x; ni[3] = b.y;
     const uint4 g0 = philox4x32_10(make_uint4(f_lo, f_hi, 2u * q, 8u + j), p.seed_lo, p.seed_hi);
     const uint4 g1 = philox4x32_10(make_uint4(f_lo, f_hi, 2u * q + 1u, 8u + j), p.seed_lo, p.seed_hi);
-    hh[0] = fading_gain(p, box_muller(g0.x, g0.y)); hh[1] = fading_gain(p, box_muller(g0.z, g0.w));
-    hh[2] = fading_gain(p, box_muller(g1.x, g1.y)); hh[3] = fading_gain(p, box_muller(g1.z, g1.w));
+    hh[0] = fading_gain(p.nlos_std, p.mean_re, p.mean_im, box_muller(g0.x, g0.y));
+    hh[1] = fading_gain(p.nlos_std, p.mean_re, p.mean_im, box_muller(g0.z, g0.w));
+    hh[2] = fading_gain(p.nlos_std, p.mean_re, p.mean_im, box_muller(g1.x, g1.y));
+    hh[3] = fading_gain(p.nlos_std, p.mean_re, p.mean_im, box_muller(g1.z, g1.w));
 }
 
 // message bits: one thread per 128 bits

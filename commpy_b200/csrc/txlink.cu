@@ -8,14 +8,12 @@
 // message bits are returned, and the receiver (cpb_demod_soft -> cpb_viterbi_decode -> cpb_count_errors) is what is
 // checked against the oracle.
 //
-// Randomness is counter based (Philox4x32-10): message bit i of global frame f is bit (i & 127) of
-// Philox(counter = (f_lo, f_hi, i >> 7, 0), key = seed); the noise of symbols 2q, 2q+1 of frame f comes from
-// Philox(counter = (f_lo, f_hi, q, 1), key = seed) through Box-Muller.  Results therefore do not depend on the launch
-// geometry, the batch split or the number of GPUs (each rank passes its own first_frame), SURVEY 8(e).
+// Randomness is counter based (Philox4x32-10), so results do not depend on the launch geometry, the batch split or the
+// number of GPUs, SURVEY 8(e): the message, noise and gain streams are the counter words of philox.cuh.
 //
-// Flat fading (FADING = true, cpb_conv_link_tx_fading; SISOFlatChannel, commpy/channels.py:176-221): the gains of symbols
-// 2q, 2q+1 of frame f come from Philox(counter = (f_lo, f_hi, q, 5), key = seed) through the same Box-Muller,
-// h = los + nlos_std (g.x + j g.y), and y = h c + sigma n with the noise n above; h is written out next to y.
+// Flat fading (FADING = true, cpb_conv_link_tx_fading; SISOFlatChannel, commpy/channels.py:176-221): each symbol c gets
+// its own gain h = los + nlos_std (g.x + j g.y), and y = h c + sigma n with the AWGN link's noise n; h is written out
+// next to y.
 //
 // Encoder: k = 1 feed-forward shift register; tap mask g_j bit b multiplies the input delayed by b (bit 0 = current
 // input) -- derived on the host from the Trellis tables and verified against every (state, input) entry.
@@ -23,6 +21,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "philox.cuh"
 
 using namespace cpb;
 
@@ -53,35 +52,6 @@ struct Params {
     float nlos_std;
     float2 *h;                // fading gains, same layout as y
 };
-
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1)
-{
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-        c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    return c;
-}
-
-// two uint32 -> two standard normals (Box-Muller); u1 in (0, 1]
-__device__ __forceinline__ float2 box_muller(uint32_t a, uint32_t b)
-{
-    const float u1 = fmaf((float)a, 2.3283064365386963e-10f, 1.1641532182693481e-10f);
-    const float u2 = (float)b * 2.3283064365386963e-10f;
-    const float r = sqrtf(-2.0f * __logf(u1));
-    float sn, cs;
-    __sincosf(6.283185307179586f * u2, &sn, &cs);
-    return make_float2(r * cs, r * sn);
-}
-
-// fading gain of one symbol from two standard normals
-__device__ __forceinline__ float2 fading_gain(const Params &p, float2 g)
-{
-    return make_float2(fmaf(p.nlos_std, g.x, p.los_re), fmaf(p.nlos_std, g.y, p.los_im));
-}
 
 // h * c; exact at h = 1 + 0j (1 * c.x - 0 * c.y is c.x whichever product the compiler fuses)
 __device__ __forceinline__ float2 cmul(float2 h, float2 c)
@@ -137,8 +107,8 @@ __global__ void __launch_bounds__(128) conv_link_tx_kernel(const Params p)
         float2 h;
         if ((s & 1) == 0 || s == s0) {
             const uint4 r = philox4x32_10(make_uint4(f_lo, f_hi, (uint32_t)(s >> 1), 5u), p.seed_lo, p.seed_hi);
-            h = fading_gain(p, box_muller(r.x, r.y));
-            hspare = fading_gain(p, box_muller(r.z, r.w));
+            h = fading_gain(p.nlos_std, p.los_re, p.los_im, box_muller(r.x, r.y));
+            hspare = fading_gain(p.nlos_std, p.los_re, p.los_im, box_muller(r.z, r.w));
             if (s & 1) h = hspare;
         } else {
             h = hspare;
@@ -258,7 +228,8 @@ __global__ void __launch_bounds__(128) conv_link_tx_fast_kernel(const Params p)
             float2 a0 = s_map[k0], a1 = s_map[k1];
             if (FADING) {
                 const uint4 rh = philox4x32_10(make_uint4(f_lo, f_hi, gs >> 1, 5u), p.seed_lo, p.seed_hi);
-                const float2 h0 = fading_gain(p, box_muller(rh.x, rh.y)), h1 = fading_gain(p, box_muller(rh.z, rh.w));
+                const float2 h0 = fading_gain(p.nlos_std, p.los_re, p.los_im, box_muller(rh.x, rh.y));
+                const float2 h1 = fading_gain(p.nlos_std, p.los_re, p.los_im, box_muller(rh.z, rh.w));
                 *reinterpret_cast<float4 *>(p.h + (y - p.y) + sym) = make_float4(h0.x, h0.y, h1.x, h1.y);
                 a0 = cmul(h0, a0);
                 a1 = cmul(h1, a1);

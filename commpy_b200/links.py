@@ -223,30 +223,7 @@ def conv_link_tx(trellis, modem, frames, frame_bits, seed, first_frame, noise_si
     Returns (msg uint8 (frames, frame_bits), y complex64 (frames, frame_bits*n/bits_per_symbol)) as CUDA tensors.
     The streams depend only on (seed, global frame index): any split of the frames over calls or ranks gives the
     same frames."""
-    import ctypes as C
-    from .channelcoding.convcode import _trellis_handle
-    torch = _lib.require_cuda()
-    nb = int(modem.num_bits_symbol)
-    kept = kept_bits(int(trellis.n) * int(frame_bits), puncture)
-    if kept % nb:
-        raise ValueError("the (punctured) coded bits of a frame must fill whole symbols")
-    nsym = kept // nb
-    msg = torch.empty((int(frames), int(frame_bits)), dtype=torch.uint8, device="cuda")
-    y = torch.empty((int(frames), nsym), dtype=torch.complex64, device="cuda")
-    if puncture is None:
-        rc = _lib.load().cpb_conv_link_tx(_trellis_handle(trellis), modem._handle(), C.c_int64(int(frames)),
-                                          C.c_int64(int(frame_bits)), C.c_uint64(int(seed) & ((1 << 64) - 1)),
-                                          C.c_int64(int(first_frame)), C.c_float(float(noise_sigma)), _lib.ptr(msg),
-                                          _lib.ptr(y), _lib.stream_ptr(torch))
-    else:
-        pv = np.ascontiguousarray(puncture, dtype=np.int32)
-        rc = _lib.load().cpb_conv_link_tx_punctured(_trellis_handle(trellis), modem._handle(), C.c_int64(int(frames)),
-                                                    C.c_int64(int(frame_bits)), C.c_uint64(int(seed) & ((1 << 64) - 1)),
-                                                    C.c_int64(int(first_frame)), C.c_float(float(noise_sigma)),
-                                                    _lib.ptr(pv), int(len(pv)), _lib.ptr(msg), _lib.ptr(y),
-                                                    _lib.stream_ptr(torch))
-    _lib.check(rc, "conv_link_tx")
-    return msg, y
+    return _conv_link_tx(trellis, modem, frames, frame_bits, seed, first_frame, noise_sigma, None, puncture)
 
 
 def _fading(fading_param):
@@ -267,27 +244,51 @@ def conv_link_tx_fading(trellis, modem, frames, frame_bits, seed, first_frame, n
     the streams of `conv_link_tx` (at fading_param = (1 + 0j, 0) the outputs are identical to it).
 
     Returns (msg uint8 (frames, frame_bits), y complex64 (frames, nsym), h complex64 (frames, nsym)) as CUDA tensors."""
+    return _conv_link_tx(trellis, modem, frames, frame_bits, seed, first_frame, noise_sigma, fading_param, puncture)
+
+
+def _conv_link_tx(trellis, modem, frames, frame_bits, seed, first_frame, noise_sigma, fading_param, puncture):
+    """conv_link_tx (fading_param None: AWGN, (msg, y)) and conv_link_tx_fading ((msg, y, h)).  AWGN calls the AWGN entry
+    points, which launch the kernels without the fading code."""
     import ctypes as C
     from .channelcoding.convcode import _trellis_handle
-    mean, nlos = _fading(fading_param)
+    if fading_param is not None:
+        mean, nlos = _fading(fading_param)
     torch = _lib.require_cuda()
     nb = int(modem.num_bits_symbol)
     kept = kept_bits(int(trellis.n) * int(frame_bits), puncture)
     if kept % nb:
         raise ValueError("the (punctured) coded bits of a frame must fill whole symbols")
-    nsym = kept // nb
-    msg = torch.empty((int(frames), int(frame_bits)), dtype=torch.uint8, device="cuda")
-    y = torch.empty((int(frames), nsym), dtype=torch.complex64, device="cuda")
-    h = torch.empty((int(frames), nsym), dtype=torch.complex64, device="cuda")
+    frames, frame_bits = int(frames), int(frame_bits)
+    msg = torch.empty((frames, frame_bits), dtype=torch.uint8, device="cuda")
+    y = torch.empty((frames, kept // nb), dtype=torch.complex64, device="cuda")
     pv = None if puncture is None else np.ascontiguousarray(puncture, dtype=np.int32)
-    rc = _lib.load().cpb_conv_link_tx_fading(_trellis_handle(trellis), modem._handle(), C.c_int64(int(frames)),
-                                             C.c_int64(int(frame_bits)), C.c_uint64(int(seed) & ((1 << 64) - 1)),
-                                             C.c_int64(int(first_frame)), C.c_float(float(noise_sigma)),
-                                             C.c_float(mean.real), C.c_float(mean.imag), C.c_float(nlos), _lib.ptr(pv),
-                                             0 if pv is None else int(len(pv)), _lib.ptr(msg), _lib.ptr(y), _lib.ptr(h),
-                                             _lib.stream_ptr(torch))
-    _lib.check(rc, "conv_link_tx_fading")
-    return msg, y, h
+    lib = _lib.load()
+    head = (_trellis_handle(trellis), modem._handle(), C.c_int64(frames), C.c_int64(frame_bits),
+            C.c_uint64(int(seed) & ((1 << 64) - 1)), C.c_int64(int(first_frame)), C.c_float(float(noise_sigma)))
+    if fading_param is not None:
+        h = torch.empty_like(y)
+        rc = lib.cpb_conv_link_tx_fading(*head, C.c_float(mean.real), C.c_float(mean.imag), C.c_float(nlos), _lib.ptr(pv),
+                                         0 if pv is None else len(pv), _lib.ptr(msg), _lib.ptr(y), _lib.ptr(h),
+                                         _lib.stream_ptr(torch))
+        _lib.check(rc, "conv_link_tx_fading")
+        return msg, y, h
+    if pv is None:
+        rc = lib.cpb_conv_link_tx(*head, _lib.ptr(msg), _lib.ptr(y), _lib.stream_ptr(torch))
+    else:
+        rc = lib.cpb_conv_link_tx_punctured(*head, _lib.ptr(pv), len(pv), _lib.ptr(msg), _lib.ptr(y), _lib.stream_ptr(torch))
+    _lib.check(rc, "conv_link_tx")
+    return msg, y
+
+
+def _count_errors(dec, msg, counters, torch):
+    """cpb_count_errors: adds the bit errors and the frames with an error of the decoded rows `dec` against the first
+    msg.shape[1] bits of each row to `counters` (device side, no sync)"""
+    import ctypes as C
+    L = msg.shape[1]
+    rc = _lib.load().cpb_count_errors(_lib.ptr(dec), _lib.ptr(msg), C.c_int64(msg.shape[0]), C.c_int64(L),
+                                      C.c_int64(dec.shape[1]), C.c_int64(L), _lib.ptr(counters), _lib.stream_ptr(torch))
+    _lib.check(rc, "count_errors")
 
 
 def kept_bits(n_coded, puncture):
@@ -354,7 +355,6 @@ class ConvLinkGPU:
 
     # -- RX chain: this package's kernels -------------------------------------------------------------
     def receive_decode_count(self, msg, y, noise_var, counters, torch, channel_gains=None):
-        import ctypes as C
         from .channelcoding import viterbi_decode_batch
         if self.decoding_type == "soft":
             rx = self.modem.demodulate_batch(y, "soft", noise_var, channel_gains)
@@ -366,10 +366,7 @@ class ConvLinkGPU:
             from .channelcoding import viterbi_decode_punctured_batch
             dec = viterbi_decode_punctured_batch(rx, self.trellis, self.puncture, self.trellis.n * self.frame_bits,
                                                  self.tb_depth, "soft")
-        L = msg.shape[1]
-        rc = _lib.load().cpb_count_errors(_lib.ptr(dec), _lib.ptr(msg), C.c_int64(msg.shape[0]), C.c_int64(L),
-                                          C.c_int64(dec.shape[1]), C.c_int64(L), _lib.ptr(counters), _lib.stream_ptr(torch))
-        _lib.check(rc, "count_errors")
+        _count_errors(dec, msg, counters, torch)
         return dec
 
     def link_performance(self, SNRs, send_max, err_min, return_counters=False, stop_early=True, overlap_points=True):
@@ -461,20 +458,7 @@ def turbo_link_tx(trellis, interleaver, frames, frame_bits, seed, first_frame, n
 
     Returns (msg uint8, sys, par1, par2 float32), each (frames, frame_bits), CUDA tensors: what map_decode / turbo_decode
     take.  The streams depend only on (seed, global frame index)."""
-    import ctypes as C
-    from .channelcoding.convcode import _trellis_handle
-    from .channelcoding.turbo import _checked_perm
-    torch = _lib.require_cuda()
-    N = int(frame_bits)
-    perm = torch.from_numpy(_checked_perm(interleaver, N)).cuda()
-    msg = torch.empty((int(frames), N), dtype=torch.uint8, device="cuda")
-    ys, y1, y2 = (torch.empty((int(frames), N), dtype=torch.float32, device="cuda") for _ in range(3))
-    rc = _lib.load().cpb_turbo_link_tx(_trellis_handle(trellis), _lib.ptr(perm), C.c_int64(int(frames)), C.c_int64(N),
-                                       C.c_uint64(int(seed) & ((1 << 64) - 1)), C.c_int64(int(first_frame)),
-                                       C.c_float(float(noise_sigma)), _lib.ptr(msg), _lib.ptr(ys), _lib.ptr(y1), _lib.ptr(y2),
-                                       _lib.stream_ptr(torch))
-    _lib.check(rc, "turbo_link_tx")
-    return msg, ys, y1, y2
+    return _turbo_link_tx(trellis, interleaver, frames, frame_bits, seed, first_frame, noise_sigma, None)
 
 
 def turbo_link_tx_fading(trellis, interleaver, frames, frame_bits, seed, first_frame, noise_sigma, fading_param):
@@ -486,21 +470,34 @@ def turbo_link_tx_fading(trellis, interleaver, frames, frame_bits, seed, first_f
     Returns (msg uint8 (frames, frame_bits), y complex64 (3, frames, frame_bits), h complex64 (3, frames, frame_bits)) as
     CUDA tensors; stream 0 is systematic, 1 and 2 the parity streams.  `bpsk_combine(y, h)` gives what turbo_decode
     takes at noise_variance = noise_sigma ** 2."""
+    return _turbo_link_tx(trellis, interleaver, frames, frame_bits, seed, first_frame, noise_sigma, fading_param)
+
+
+def _turbo_link_tx(trellis, interleaver, frames, frame_bits, seed, first_frame, noise_sigma, fading_param):
+    """turbo_link_tx (fading_param None: AWGN, (msg, sys, par1, par2)) and turbo_link_tx_fading ((msg, y, h))."""
     import ctypes as C
     from .channelcoding.convcode import _trellis_handle
     from .channelcoding.turbo import _checked_perm
-    mean, nlos = _fading(fading_param)
+    if fading_param is not None:
+        mean, nlos = _fading(fading_param)
     torch = _lib.require_cuda()
     N = int(frame_bits)
     perm = torch.from_numpy(_checked_perm(interleaver, N)).cuda()
-    msg = torch.empty((int(frames), N), dtype=torch.uint8, device="cuda")
-    y, h = (torch.empty((3, int(frames), N), dtype=torch.complex64, device="cuda") for _ in range(2))
-    rc = _lib.load().cpb_turbo_link_tx_fading(_trellis_handle(trellis), _lib.ptr(perm), C.c_int64(int(frames)), C.c_int64(N),
-                                              C.c_uint64(int(seed) & ((1 << 64) - 1)), C.c_int64(int(first_frame)),
-                                              C.c_float(float(noise_sigma)), C.c_float(mean.real), C.c_float(mean.imag),
-                                              C.c_float(nlos), _lib.ptr(msg), _lib.ptr(y), _lib.ptr(h), _lib.stream_ptr(torch))
-    _lib.check(rc, "turbo_link_tx_fading")
-    return msg, y, h
+    frames = int(frames)
+    msg = torch.empty((frames, N), dtype=torch.uint8, device="cuda")
+    lib = _lib.load()
+    head = (_trellis_handle(trellis), _lib.ptr(perm), C.c_int64(frames), C.c_int64(N),
+            C.c_uint64(int(seed) & ((1 << 64) - 1)), C.c_int64(int(first_frame)), C.c_float(float(noise_sigma)))
+    if fading_param is not None:
+        y, h = (torch.empty((3, frames, N), dtype=torch.complex64, device="cuda") for _ in range(2))
+        rc = lib.cpb_turbo_link_tx_fading(*head, C.c_float(mean.real), C.c_float(mean.imag), C.c_float(nlos), _lib.ptr(msg),
+                                          _lib.ptr(y), _lib.ptr(h), _lib.stream_ptr(torch))
+        _lib.check(rc, "turbo_link_tx_fading")
+        return msg, y, h
+    ys, y1, y2 = (torch.empty((frames, N), dtype=torch.float32, device="cuda") for _ in range(3))
+    rc = lib.cpb_turbo_link_tx(*head, _lib.ptr(msg), _lib.ptr(ys), _lib.ptr(y1), _lib.ptr(y2), _lib.stream_ptr(torch))
+    _lib.check(rc, "turbo_link_tx")
+    return msg, ys, y1, y2
 
 
 def bpsk_combine(y, h):
@@ -554,7 +551,6 @@ class TurboLinkGPU:
     def decode_count(self, msg, *args):
         """decode_count(*make_batch(...), counters, torch): decode(msg, sys, par1, par2, s2, counters, torch) over AWGN,
         (msg, y, h, s2, counters, torch) over fading -- y and h are combined first.  Adds the errors to `counters`."""
-        import ctypes as C
         from .channelcoding import turbo_decode_batch
         *rx, s2, counters, torch = args
         if self.fading_param is not None:
@@ -563,10 +559,7 @@ class TurboLinkGPU:
         else:
             ys, y1, y2 = rx
         dec = turbo_decode_batch(ys, y1, y2, self.trellis, s2, self.iterations, self.interleaver)
-        L = msg.shape[1]
-        rc = _lib.load().cpb_count_errors(_lib.ptr(dec), _lib.ptr(msg), C.c_int64(msg.shape[0]), C.c_int64(L), C.c_int64(L),
-                                          C.c_int64(L), _lib.ptr(counters), _lib.stream_ptr(torch))
-        _lib.check(rc, "count_errors")
+        _count_errors(dec, msg, counters, torch)
         return dec
 
     def link_performance(self, EbN0s, send_max, err_min):

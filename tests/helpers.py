@@ -176,7 +176,7 @@ def launched_kernels(fn):
     return {normalize_kernel_name(s) for s in names if not s.startswith(("Memcpy", "Memset"))}
 
 
-# ---- NumPy model of the device-side TX chain (commpy_b200/csrc/txlink.cu) ------------------------------------------
+# ---- NumPy model of the device-side TX chains (commpy_b200/csrc/txlink.cu, turbolink.cu) ---------------------------
 def philox4x32_10(ctr, key):
     """Philox4x32-10 (Salmon et al., Random123).  ctr: (N, 4) uint32 counters, key: (k0, k1).  Returns (N, 4) uint32."""
     c = np.asarray(ctr, dtype=np.uint64).copy()
@@ -193,6 +193,36 @@ def philox4x32_10(ctr, key):
     return c.astype(np.uint32)
 
 
+def _philox_words(frame, count, word, key):
+    """Philox of the counters (f_lo, f_hi, 0 .. count-1, word) of global frame `frame`: (count, 4) uint32"""
+    ctr = np.zeros((count, 4), dtype=np.uint64)
+    ctr[:, 0], ctr[:, 1], ctr[:, 2], ctr[:, 3] = frame & 0xFFFFFFFF, frame >> 32, np.arange(count), word
+    return philox4x32_10(ctr, key)
+
+
+def philox_bits(frame, nbits, key):
+    """The first `nbits` message bits of global frame `frame` (counter word 0, 128 bits per counter, LSB first)."""
+    words = _philox_words(frame, -(-nbits // 128), 0, key).reshape(-1)
+    return ((words[:, None] >> np.arange(32, dtype=np.uint32)[None, :]) & 1).reshape(-1)[:nbits]
+
+
+def philox_normals(frame, count, word, key):
+    """Counters 0 .. count-1 of `word` through float64 Box-Muller: (count, 2) complex standard normals, g.x + j g.y of the
+    two Box-Mullers of each counter (commpy_b200/csrc/philox.cuh lists which word feeds which stream)."""
+    r = _philox_words(frame, count, word, key).astype(np.float64)
+    za = np.sqrt(-2 * np.log(r[:, 0] * 2.0 ** -32 + 2.0 ** -33)) * np.exp(2j * np.pi * r[:, 1] * 2.0 ** -32)
+    zb = np.sqrt(-2 * np.log(r[:, 2] * 2.0 ** -32 + 2.0 ** -33)) * np.exp(2j * np.pi * r[:, 3] * 2.0 ** -32)
+    return np.stack([za, zb], axis=1)
+
+
+def same(a, b):
+    """torch.equal, complex tensors compared through their real views"""
+    import torch
+    if a.is_complex():
+        a, b = torch.view_as_real(a), torch.view_as_real(b)
+    return torch.equal(a, b)
+
+
 def conv_link_tx_model(trellis, modem, frames, frame_bits, seed, first_frame, noise_sigma, puncture=None):
     """(msg, y) exactly as cpb_conv_link_tx defines them (float64 Box-Muller for the noise)."""
     key = (seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
@@ -206,25 +236,13 @@ def conv_link_tx_model(trellis, modem, frames, frame_bits, seed, first_frame, no
     cst = np.asarray(modem.constellation)
     for fl in range(frames):
         f = first_frame + fl
-        nblk = -(-frame_bits // 128)
-        ctr = np.zeros((nblk, 4), dtype=np.uint64)
-        ctr[:, 0], ctr[:, 1], ctr[:, 2], ctr[:, 3] = f & 0xFFFFFFFF, f >> 32, np.arange(nblk), 0
-        words = philox4x32_10(ctr, key).reshape(-1)                              # 32-bit words, LSB first
-        bits = ((words[:, None] >> np.arange(32, dtype=np.uint32)[None, :]) & 1).reshape(-1)[:frame_bits]
+        bits = philox_bits(f, frame_bits, key)
         msg[fl] = bits
         coded = conv_encode(bits.astype(int), trellis, "cont")
         if puncture is not None:
             coded = puncturing(coded, puncture)
         idx = coded.reshape(-1, nb).dot(1 << np.arange(nb - 1, -1, -1))
-        npair = -(-nsym // 2)
-        ctr = np.zeros((npair, 4), dtype=np.uint64)
-        ctr[:, 0], ctr[:, 1], ctr[:, 2], ctr[:, 3] = f & 0xFFFFFFFF, f >> 32, np.arange(npair), 1
-        r = philox4x32_10(ctr, key).astype(np.float64)
-        u1a, u2a = r[:, 0] * 2.0 ** -32 + 2.0 ** -33, r[:, 1] * 2.0 ** -32
-        u1b, u2b = r[:, 2] * 2.0 ** -32 + 2.0 ** -33, r[:, 3] * 2.0 ** -32
-        za = np.sqrt(-2 * np.log(u1a)) * np.exp(2j * np.pi * u2a)
-        zb = np.sqrt(-2 * np.log(u1b)) * np.exp(2j * np.pi * u2b)
-        z = np.stack([za, zb], axis=1).reshape(-1)[:nsym]
+        z = philox_normals(f, -(-nsym // 2), 1, key).reshape(-1)[:nsym]
         y[fl] = cst[idx] + noise_sigma * z
     return msg, y
 
@@ -239,23 +257,12 @@ def turbo_link_tx_model(trellis, interleaver, frames, frame_bits, seed, first_fr
     ys = np.zeros((frames, 3, N))
     for fl in range(frames):
         f = first_frame + fl
-        nblk = -(-N // 128)
-        ctr = np.zeros((nblk, 4), dtype=np.uint64)
-        ctr[:, 0], ctr[:, 1], ctr[:, 2], ctr[:, 3] = f & 0xFFFFFFFF, f >> 32, np.arange(nblk), 0
-        words = philox4x32_10(ctr, key).reshape(-1)
-        bits = ((words[:, None] >> np.arange(32, dtype=np.uint32)[None, :]) & 1).reshape(-1)[:N]
+        bits = philox_bits(f, N, key)
         msg[fl] = bits
         streams = turbo_encode(bits.astype(int), trellis, trellis, interleaver)
-        nq = -(-N // 4)
         for j in range(3):
-            ctr = np.zeros((nq, 4), dtype=np.uint64)
-            ctr[:, 0], ctr[:, 1], ctr[:, 2], ctr[:, 3] = f & 0xFFFFFFFF, f >> 32, np.arange(nq), 2 + j
-            r = philox4x32_10(ctr, key).astype(np.float64)
-            u1a, u2a = r[:, 0] * 2.0 ** -32 + 2.0 ** -33, r[:, 1] * 2.0 ** -32
-            u1b, u2b = r[:, 2] * 2.0 ** -32 + 2.0 ** -33, r[:, 3] * 2.0 ** -32
-            za = np.sqrt(-2 * np.log(u1a)) * np.exp(2j * np.pi * u2a)
-            zb = np.sqrt(-2 * np.log(u1b)) * np.exp(2j * np.pi * u2b)
-            z = np.stack([za.real, za.imag, zb.real, zb.imag], axis=1).reshape(-1)[:N]
+            z = philox_normals(f, -(-N // 4), 2 + j, key)
+            z = np.stack([z.real, z.imag], axis=2).reshape(-1)[:N]
             ys[fl, j] = (2.0 * np.asarray(streams[j][:N], dtype=np.float64) - 1.0) + noise_sigma * z
     return msg, ys[:, 0], ys[:, 1], ys[:, 2]
 

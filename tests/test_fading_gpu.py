@@ -40,14 +40,8 @@ def gains_model(frames, nsym, seed, first_frame, fading_param):
     mean, nlos = complex(fading_param[0]), float(np.real(fading_param[1]))
     h = np.zeros((frames, nsym), dtype=np.complex128)
     for fl in range(frames):
-        f = first_frame + fl
-        npair = -(-nsym // 2)
-        ctr = np.zeros((npair, 4), dtype=np.uint64)
-        ctr[:, 0], ctr[:, 1], ctr[:, 2], ctr[:, 3] = f & 0xFFFFFFFF, f >> 32, np.arange(npair), 5
-        r = helpers.philox4x32_10(ctr, key).astype(np.float64)
-        za = np.sqrt(-2 * np.log(r[:, 0] * 2.0 ** -32 + 2.0 ** -33)) * np.exp(2j * np.pi * r[:, 1] * 2.0 ** -32)
-        zb = np.sqrt(-2 * np.log(r[:, 2] * 2.0 ** -32 + 2.0 ** -33)) * np.exp(2j * np.pi * r[:, 3] * 2.0 ** -32)
-        h[fl] = mean + math.sqrt(nlos / 2) * np.stack([za, zb], axis=1).reshape(-1)[:nsym]
+        g = helpers.philox_normals(first_frame + fl, -(-nsym // 2), 5, key)
+        h[fl] = mean + math.sqrt(nlos / 2) * g.reshape(-1)[:nsym]
     return h
 
 
@@ -99,13 +93,6 @@ def _tx_both(fn):
     return out
 
 
-def _same(a, b):
-    import torch
-    if a.is_complex():
-        a, b = torch.view_as_real(a), torch.view_as_real(b)
-    return torch.equal(a, b)
-
-
 @gpu
 def test_unit_gain_equals_awgn_link_bit_for_bit():
     """fading_param = (1 + 0j, 0): msg and y equal cpb_conv_link_tx[_punctured] bit for bit and h == 1, for the word-parallel
@@ -118,7 +105,8 @@ def test_unit_gain_equals_awgn_link_bit_for_bit():
         awgn = _tx_both(lambda: conv_link_tx(tr, modem, 9, fb, seed, first, 0.6, punct))
         fad = _tx_both(lambda: conv_link_tx_fading(tr, modem, 9, fb, seed, first, 0.6, (1 + 0j, 0), punct))
         for force in (0, 1):
-            assert _same(fad[force][0], awgn[force][0]) and _same(fad[force][1], awgn[force][1]), (fb, punct, force)
+            assert helpers.same(fad[force][0], awgn[force][0]), (fb, punct, force)
+            assert helpers.same(fad[force][1], awgn[force][1]), (fb, punct, force)
             h = fad[force][2].cpu().numpy()
             assert h.shape == awgn[force][1].shape and (h == 1).all()
 
@@ -135,7 +123,7 @@ def test_fading_word_parallel_kernel_equals_bit_serial(modem_m):
     for tr, frame_bits in ((helpers.k7(), 1024), (helpers.k7_wifi_quirk(), 128), (helpers.k7(), 4096), (k3, 256)):
         out = _tx_both(lambda: conv_link_tx_fading(tr, modem, 37, frame_bits, 0xfeedbeef12345, (1 << 32) - 5, 0.6, RAYLEIGH))
         for a, b in zip(out[0], out[1]):
-            assert _same(a, b), (modem_m, frame_bits)
+            assert helpers.same(a, b), (modem_m, frame_bits)
 
 
 @gpu
@@ -159,7 +147,7 @@ def test_fading_tx_matches_numpy_model(modem_m, frame_bits, punct):
         noise = y.cpu().numpy() - hn.astype(np.complex128) * points
         assert np.abs(noise - (y_awgn - points)).max() < 2e-3
         msg3, y3, h3 = conv_link_tx_fading(tr, modem, 3, frame_bits, seed, first + 2, sigma, fp, punct)
-        assert torch.equal(msg3, msg[2:]) and _same(y3, y[2:]) and _same(h3, h[2:])
+        assert torch.equal(msg3, msg[2:]) and helpers.same(y3, y[2:]) and helpers.same(h3, h[2:])
 
 
 @gpu

@@ -23,17 +23,6 @@ FP32_EPS = 2.0 ** -23
 
 
 # ---------------------------------------------------------------- float64 model of the streams
-def _normals(f, count, word, key):
-    """`count` Philox counters (f_lo, f_hi, c, word) through float64 Box-Muller: (count, 2) complex standard normals
-    (g.x + j g.y of the two Box-Mullers of each call, in call order)"""
-    ctr = np.zeros((count, 4), dtype=np.uint64)
-    ctr[:, 0], ctr[:, 1], ctr[:, 2], ctr[:, 3] = f & 0xFFFFFFFF, f >> 32, np.arange(count), word
-    r = helpers.philox4x32_10(ctr, key).astype(np.float64)
-    za = np.sqrt(-2 * np.log(r[:, 0] * 2.0 ** -32 + 2.0 ** -33)) * np.exp(2j * np.pi * r[:, 1] * 2.0 ** -32)
-    zb = np.sqrt(-2 * np.log(r[:, 2] * 2.0 ** -32 + 2.0 ** -33)) * np.exp(2j * np.pi * r[:, 3] * 2.0 ** -32)
-    return np.stack([za, zb], axis=1)
-
-
 def fading_model(trellis, interleaver, frames, N, seed, first_frame, fading_param):
     """(msg, x, n_re, n_im, h), each stream-major (3, frames, N) but msg, exactly as cpb_turbo_link_tx_fading defines them:
     x = 2 bit - 1 of turbo_encode's streams (helpers.turbo_link_tx_model), n_re its noise (counter word 2 + j), n_im counter
@@ -50,9 +39,9 @@ def fading_model(trellis, interleaver, frames, N, seed, first_frame, fading_para
     for fl in range(frames):
         f = first_frame + fl
         for j in range(3):
-            z = _normals(f, -(-N // 4), 5 + j, key)
+            z = helpers.philox_normals(f, -(-N // 4), 5 + j, key)
             n_im[j, fl] = np.stack([z.real, z.imag], axis=2).reshape(-1)[:N]
-            h[j, fl] = mean + math.sqrt(nlos / 2) * _normals(f, -(-N // 2), 8 + j, key).reshape(-1)[:N]
+            h[j, fl] = mean + math.sqrt(nlos / 2) * helpers.philox_normals(f, -(-N // 2), 8 + j, key).reshape(-1)[:N]
     return msg, x, n_re, n_im, h
 
 
@@ -98,13 +87,6 @@ def test_c_entry_points_reject_bad_arguments_before_any_device_call():
 
 
 # ---------------------------------------------------------------- TX kernel
-def _same(a, b):
-    import torch
-    if a.is_complex():
-        a, b = torch.view_as_real(a), torch.view_as_real(b)
-    return torch.equal(a, b)
-
-
 @gpu
 @pytest.mark.parametrize("N", [256, 1000, 6144])
 def test_unit_gain_equals_awgn_link_bit_for_bit(N):
@@ -156,7 +138,7 @@ def test_fading_tx_matches_numpy_model(N):
         msg2, y2, h2 = turbo_link_tx_fading(tr, il, 2, N, seed, first, sigma, fp)
         msg3, y3, h3 = turbo_link_tx_fading(tr, il, 3, N, seed, first + 2, sigma, fp)
         assert torch.equal(torch.cat([msg2, msg3]), msg)
-        assert _same(torch.cat([y2, y3], dim=1), y) and _same(torch.cat([h2, h3], dim=1), h)
+        assert helpers.same(torch.cat([y2, y3], dim=1), y) and helpers.same(torch.cat([h2, h3], dim=1), h)
 
 
 @gpu
