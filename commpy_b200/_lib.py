@@ -15,6 +15,7 @@ CPB_U8, CPB_F32 = 0, 1
 VITERBI_MODES = {"hard": 0, "soft": 1, "unquantized": 2}
 LDPC_FP32, LDPC_FP64 = 0, 1
 OPT_VITERBI_FORCE_GENERIC, OPT_LDPC_NO_BULK, OPT_BCJR_WINDOW, OPT_BCJR_PER_STEP_SCALING, OPT_TURBO_FRAME_MAJOR, OPT_TX_FORCE_GENERIC = 0, 1, 2, 3, 4, 5
+OPT_LDPC_ENC_FORCE_DENSE = 6
 
 # every symbol include/commpy_b200.h declares (tests/test_abi.py checks the header against this list)
 SYMBOLS = [
@@ -29,6 +30,7 @@ SYMBOLS = [
     "cpb_demod_soft_csi", "cpb_demod_hard_csi",
     "cpb_count_errors", "cpb_conv_link_tx", "cpb_conv_link_tx_punctured", "cpb_conv_link_tx_fading", "cpb_turbo_link_tx",
     "cpb_turbo_link_tx_fading", "cpb_bpsk_combine",
+    "cpb_ldpc_encode", "cpb_ldpc_encoder_plan", "cpb_ldpc_link_tx", "cpb_ldpc_link_tx_fading",
 ]
 
 _lib = None

@@ -11,7 +11,7 @@ import scipy.sparse as sp
 from .. import _lib
 
 __all__ = ["build_matrix", "get_ldpc_code_params", "ldpc_bp_decode", "ldpc_bp_decode_batch", "write_ldpc_params",
-           "triang_ldpc_systematic_encode"]
+           "triang_ldpc_systematic_encode", "ldpc_encode_batch"]
 
 _llr_max = 500
 
@@ -101,6 +101,41 @@ def _ldpc_handle(ldpc_code_params):
         _lib.check(rc, "ldpc parity-check matrix")
         cache[dev] = (_LdpcBox(h), H.shape[1])
     return cache[dev][0].ptr, cache[dev][1]
+
+
+def _code_dims(ldpc_code_params):
+    """(n, m) of a code dict, from its parity-check matrix when it has one, else from its design-file fields"""
+    H = ldpc_code_params.get("parity_check_matrix")
+    if H is not None:
+        return int(H.shape[1]), int(H.shape[0])
+    return int(ldpc_code_params["n_vnodes"]), int(ldpc_code_params["n_cnodes"])
+
+
+def ldpc_encode_batch(msg, ldpc_code_params):
+    """Systematic LDPC encoding on the GPU (cpb_ldpc_encode) of a (batch, k) array of message bits, k = n - m.
+
+    msg : torch tensor (CUDA or host) or numpy array of 0/1 values.  Returns the (batch, n) uint8 code words
+    [message | parity] with H c = 0 over GF(2), as a torch CUDA tensor.  The parity is p = H_p^-1 H_s msg with
+    H = [H_s | H_p], H_p the last m columns, computed by peeling when H_p allows it and through the dense GF(2) inverse
+    otherwise (DESIGN.md section 4.7).  Where H_p is invertible over GF(2) the parity of a message is unique, so this is
+    what triang_ldpc_systematic_encode returns whenever the reference's encoding is a code word.
+    Raises ValueError for a wrong shape, values other than 0/1 or an H_p that is singular over GF(2), and
+    NotImplementedError for a code whose H_p does not peel and whose dense inverse (k * m bits) exceeds 2^26 bits.
+    A dict given only as a parity_check_matrix is used as it is: no generator matrix is computed."""
+    torch = _lib.require_cuda()
+    handle, n = _ldpc_handle(ldpc_code_params)
+    k = n - _code_dims(ldpc_code_params)[1]
+    x = msg if hasattr(msg, "data_ptr") else torch.from_numpy(np.ascontiguousarray(msg))
+    if x.dim() != 2 or x.shape[1] != k:
+        raise ValueError("msg must be (batch, k) = (batch, %d), got %s" % (k, tuple(x.shape)))
+    x = x.cuda()
+    if x.numel() and bool(((x != 0) & (x != 1)).any()):
+        raise ValueError("msg must hold 0/1 values")
+    x = x.to(torch.uint8).contiguous()
+    cw = torch.empty((x.shape[0], n), dtype=torch.uint8, device=x.device)
+    rc = _lib.load().cpb_ldpc_encode(handle, _lib.ptr(x), C.c_int64(x.shape[0]), _lib.ptr(cw), _lib.stream_ptr(torch))
+    _lib.check(rc, "ldpc_encode (H_p = H[:, k:] must be invertible over GF(2))")
+    return cw
 
 
 def ldpc_bp_decode_batch(llr, ldpc_code_params, n_iters, precision="fp32", return_llrs=True, return_iters=False,

@@ -47,3 +47,27 @@ struct cpbTrellis {
     int device = 0;
     cpb::PipeCtx pipe;                         // host-buffer pipeline of cpb_*_host calls made with this handle
 };
+
+namespace cpb {
+
+// Systematic LDPC encoder plans of one code (ldpclink.cu), built on first use: [0] peeled, [1] dense.  status < 0: not
+// built yet, else the cpb status the build returned (a singular code is refused on every call without redoing the work).
+struct LdpcEncPlan;
+struct LdpcEncCache {
+    std::mutex mu;
+    LdpcEncPlan *plan[2] = {nullptr, nullptr};
+    int status[2] = {-1, -1};
+    ~LdpcEncCache();
+};
+
+}  // namespace cpb
+
+struct cpbLdpc {
+    cpb::PipeCtx pipe;                                  // host-buffer pipeline of cpb_ldpc_*_host calls made with this handle
+    int m, n, nnz;
+    int max_row_deg, max_col_deg;
+    int32_t *row_ptr = nullptr, *col_idx = nullptr;     // CSR
+    int32_t *col_ptr = nullptr, *col_edge = nullptr;    // CSC: edge ids (CSR positions) of a column, ascending check
+    std::vector<int32_t> host_row_ptr, host_col_idx;    // host copy of the CSR, for the encoder plan
+    cpb::LdpcEncCache enc;
+};

@@ -30,14 +30,6 @@
 
 using namespace cpb;
 
-struct cpbLdpc {
-    cpb::PipeCtx pipe;                                  // host-buffer pipeline of cpb_ldpc_*_host calls made with this handle
-    int m, n, nnz;
-    int max_row_deg, max_col_deg;
-    int32_t *row_ptr = nullptr, *col_idx = nullptr;     // CSR
-    int32_t *col_ptr = nullptr, *col_edge = nullptr;    // CSC: edge ids (CSR positions) of a column, ascending check
-};
-
 cpb::PipeCtx &cpb_ldpc_pipe(cpbLdpc *h) { return h->pipe; }
 void cpb_ldpc_dims(const cpbLdpc *h, int *m, int *n) { *m = h->m; *n = h->n; }
 
@@ -756,6 +748,8 @@ int cpb_ldpc_create(const int32_t *row_ptr, const int32_t *col_idx, int m, int n
             col_edge[col_ptr[j] + fill[j]++] = e;
         }
     h->max_row_deg = maxr; h->max_col_deg = maxc;
+    h->host_row_ptr.assign(row_ptr, row_ptr + m + 1);
+    h->host_col_idx.assign(col_idx, col_idx + nnz);
     cudaError_t e = cudaMalloc(&h->row_ptr, sizeof(int32_t) * (m + 1));
     if (e == cudaSuccess) e = cudaMalloc(&h->col_idx, sizeof(int32_t) * nnz);
     if (e == cudaSuccess) e = cudaMalloc(&h->col_ptr, sizeof(int32_t) * (n + 1));

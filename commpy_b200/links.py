@@ -17,6 +17,9 @@
   the error counter).  With `fading_param` it runs over SISO flat fading (`turbo_link_tx_fading` ->
   cpb_turbo_link_tx_fading, one gain per coded bit), and the receiver combines coherently (`bpsk_combine` ->
   cpb_bpsk_combine, s = Re(conj(h) y)) before the unchanged turbo decoder.
+* `LdpcLinkGPU` is the batched LDPC-coded link (`ldpc_link_tx[_fading]` -> cpb_ldpc_link_tx[_fading]: Philox message,
+  systematic encoder planned from H, Modem.modulate, AWGN or flat fading), then the demapper, the LDPC decoder and the
+  error counter over the message bits.
 """
 import math
 from fractions import Fraction
@@ -27,7 +30,7 @@ import numpy as np
 from . import _lib, parallel
 
 __all__ = ["link_performance", "LinkModel", "AwgnSisoChannel", "ConvLinkGPU", "conv_link_tx", "conv_link_tx_fading",
-           "turbo_link_tx_fading", "bpsk_combine", "idd_decoder"]
+           "turbo_link_tx_fading", "bpsk_combine", "idd_decoder", "LdpcLinkGPU", "ldpc_link_tx", "ldpc_link_tx_fading"]
 
 
 class AwgnSisoChannel:
@@ -450,6 +453,107 @@ class ConvLinkGPU:
         if return_counters:
             return BERs, grand
         return BERs
+
+
+def ldpc_link_tx(ldpc_code_params, modem, frames, seed, first_frame, noise_sigma):
+    """Device-side TX chain of an LDPC-coded link (cpb_ldpc_link_tx) for `frames` frames starting at GLOBAL frame
+    `first_frame`: k random message bits -> ldpc_encode_batch ([message | parity]) -> modem.modulate -> + noise_sigma *
+    (N(0,1) + jN(0,1)).  The message and noise streams are those of `conv_link_tx`.
+
+    Returns (msg uint8 (frames, k), y complex64 (frames, n / bits_per_symbol)) as CUDA tensors."""
+    return _ldpc_link_tx(ldpc_code_params, modem, frames, seed, first_frame, noise_sigma, None)
+
+
+def ldpc_link_tx_fading(ldpc_code_params, modem, frames, seed, first_frame, noise_sigma, fading_param):
+    """`ldpc_link_tx` over SISO flat fading (cpb_ldpc_link_tx_fading): each symbol c is received as y = h c + noise with its
+    own gain h = fading_param[0] + sqrt(fading_param[1] / 2) * (N(0,1) + jN(0,1)), drawn as `conv_link_tx_fading` draws
+    them.  At fading_param = (1 + 0j, 0) the outputs equal `ldpc_link_tx`'s bit for bit.
+
+    Returns (msg uint8 (frames, k), y complex64 (frames, nsym), h complex64 (frames, nsym)) as CUDA tensors."""
+    return _ldpc_link_tx(ldpc_code_params, modem, frames, seed, first_frame, noise_sigma, fading_param)
+
+
+def _ldpc_link_tx(ldpc_code_params, modem, frames, seed, first_frame, noise_sigma, fading_param):
+    import ctypes as C
+    from .channelcoding.ldpc import _code_dims, _ldpc_handle
+    if fading_param is not None:
+        mean, nlos = _fading(fading_param)
+    n, m = _code_dims(ldpc_code_params)
+    nb = int(modem.num_bits_symbol)
+    if n % nb:
+        raise ValueError("the code words must fill whole symbols: n = %d is not a multiple of %d bits per symbol" % (n, nb))
+    torch = _lib.require_cuda()
+    handle, _ = _ldpc_handle(ldpc_code_params)
+    frames = int(frames)
+    msg = torch.empty((frames, n - m), dtype=torch.uint8, device="cuda")
+    y = torch.empty((frames, n // nb), dtype=torch.complex64, device="cuda")
+    lib = _lib.load()
+    head = (handle, modem._handle(), C.c_int64(frames), C.c_uint64(int(seed) & ((1 << 64) - 1)), C.c_int64(int(first_frame)),
+            C.c_float(float(noise_sigma)))
+    if fading_param is not None:
+        h = torch.empty_like(y)
+        rc = lib.cpb_ldpc_link_tx_fading(*head, C.c_float(mean.real), C.c_float(mean.imag), C.c_float(nlos), _lib.ptr(msg),
+                                         _lib.ptr(y), _lib.ptr(h), _lib.stream_ptr(torch))
+        _lib.check(rc, "ldpc_link_tx_fading")
+        return msg, y, h
+    rc = lib.cpb_ldpc_link_tx(*head, _lib.ptr(msg), _lib.ptr(y), _lib.stream_ptr(torch))
+    _lib.check(rc, "ldpc_link_tx")
+    return msg, y
+
+
+class LdpcLinkGPU(ConvLinkGPU):
+    """Batched LDPC-coded link on the GPU(s): frames generated and encoded on the device (cpb_ldpc_link_tx[_fading]),
+    demapped (Modem.demodulate_batch, with the channel gains over fading), decoded (ldpc_bp_decode_batch) and counted over
+    the k message bits (cpb_count_errors).  `link_performance`, `noise_std`, the counters, the stop rule and the rank
+    sharding are ConvLinkGPU's.
+
+    Parameters: `ldpc_code_params` (a design-file dict or a dict with a 'parity_check_matrix'; H_p = H[:, k:] must be
+    invertible over GF(2)), `modem` (n must be a multiple of its bits per symbol), `frames_per_batch` frames per step and
+    rank, `n_iters` / `decoder_algorithm` ('MSA' or 'SPA') / `precision` ('fp32' or 'fp64') of the decoder, `seed`, and
+    `fading_param` as for ConvLinkGPU (None: AWGN).  rate = k / n."""
+
+    def __init__(self, ldpc_code_params, modem, frames_per_batch, n_iters=15, decoder_algorithm="MSA", precision="fp32", seed=0,
+                 fading_param=None):
+        from .channelcoding.ldpc import _code_dims
+        self.fading_param = fading_param
+        if fading_param is not None:
+            _fading(fading_param)
+        if decoder_algorithm not in ("MSA", "SPA"):
+            raise ValueError("decoder_algorithm must be 'MSA' or 'SPA'")
+        if precision not in ("fp32", "fp64"):
+            raise ValueError("precision must be 'fp32' or 'fp64'")
+        n, m = _code_dims(ldpc_code_params)
+        if n % modem.num_bits_symbol:
+            raise ValueError("the code words must fill whole symbols: n = %d is not a multiple of %d bits per symbol"
+                             % (n, modem.num_bits_symbol))
+        self.params, self.modem = ldpc_code_params, modem
+        self.n, self.frame_bits, self.frames = n, n - m, int(frames_per_batch)
+        self.n_iters, self.decoder_algorithm, self.precision, self.seed = int(n_iters), decoder_algorithm, precision, int(seed)
+        self.rate = Fraction(n - m, n)
+
+    def make_batch(self, snr_db, batch_index, torch=None):
+        """(msg bits, received symbols, noise_var) for one batch of this rank -- and, over fading, the channel gains."""
+        rank, world, _ = parallel.world()
+        first = parallel.batch_first_frame(batch_index, self.frames, rank, max(world, 1))
+        ns = self.noise_std(snr_db)
+        if self.fading_param is not None:
+            msg, y, h = ldpc_link_tx_fading(self.params, self.modem, self.frames, self.seed, first, 0.5 * ns, self.fading_param)
+            return msg, y, ns ** 2, h
+        msg, y = ldpc_link_tx(self.params, self.modem, self.frames, self.seed, first, 0.5 * ns)
+        return msg, y, ns ** 2
+
+    def llrs(self, y, noise_var, channel_gains=None):
+        """decoder-convention LLRs (positive favours 0, bit = signbit(llr)) of the received symbols: the demapper's
+        log P(1) / P(0), negated.  (frames, n), float32 or float64 as the precision."""
+        llr = self.modem.demodulate_batch(y, "soft", noise_var, channel_gains).neg_()
+        return llr.double() if self.precision == "fp64" else llr
+
+    def receive_decode_count(self, msg, y, noise_var, counters, torch, channel_gains=None):
+        from .channelcoding import ldpc_bp_decode_batch
+        dec = ldpc_bp_decode_batch(self.llrs(y, noise_var, channel_gains), self.params, self.n_iters, self.precision,
+                                   return_llrs=False, decoder_algorithm=self.decoder_algorithm)
+        _count_errors(dec, msg, counters, torch)
+        return dec
 
 
 def turbo_link_tx(trellis, interleaver, frames, frame_bits, seed, first_frame, noise_sigma):

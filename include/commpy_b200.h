@@ -56,6 +56,8 @@ int cpb_release_scratch(void);
 #define CPB_OPT_TURBO_FRAME_MAJOR 4       /* 1: turbo loop on frame-major arrays with separate interleaver kernels (the cross-check
                                              of the default, which transposes once and indexes rows through the interleaver) */
 #define CPB_OPT_TX_FORCE_GENERIC 5        /* 1: cpb_conv_link_tx always runs the bit-serial kernel (cross-check of the word-parallel one) */
+#define CPB_OPT_LDPC_ENC_FORCE_DENSE 6    /* 1: the LDPC encoder uses its dense form for a peelable code that fits the dense bound
+                                             (cross-check of the peeled form) */
 #define CPB_OPT_COUNT 8
 int cpb_set_option(int option_id, int value);
 int cpb_get_option(int option_id, int *value);
@@ -264,6 +266,39 @@ int cpb_turbo_link_tx_fading(const cpbTrellis *t, const int32_t *perm_dev, int64
  * cpb_map_decode / cpb_turbo_decode take s with noise_variance = sigma^2 and decode exactly.  s = Re(y) where h = 1 + 0j,
  * 0 where h = 0. */
 int cpb_bpsk_combine(const float *y_dev, const float *h_dev, int64_t n, float *s_dev, void *stream);
+
+/* ---- LDPC systematic encoding and the transmit side of an LDPC-coded link: commpy/channelcoding/ldpc.py:302-354
+ * (triang_ldpc_systematic_encode) + Modem.modulate + AWGN / SISO flat fading (channels.py:176-221) ---- */
+/*
+ * Code words are laid out as the reference lays them out: [message (k = n - m bits) | parity (m bits)], H c = 0 over GF(2).
+ * The encoder plan is built from the handle's H on first use and freed with the handle:
+ *   peeled form when the parity part H_p = H[:, k:] peels completely (each parity bit solved in turn from one row);
+ *   dense form P = H_p^-1 H_s (GF(2)) when H_p is invertible and k * m <= 2^26.
+ * CPB_EINVAL: H_p singular over GF(2).  CPB_EUNSUPPORTED: H_p does not peel and k * m > 2^26.
+ * CPB_OPT_LDPC_ENC_FORCE_DENSE selects the dense form for a peelable code that fits the bound.
+ * msg_dev: batch x k uint8 in {0, 1} (any nonzero byte is taken as 1); cw_dev: batch x n uint8.
+ */
+int cpb_ldpc_encode(const cpbLdpc *h, const uint8_t *msg_dev, int64_t batch, uint8_t *cw_dev, void *stream);
+/* Host-only description of the plan cpb_ldpc_encode builds for H (CSR as in cpb_ldpc_create; no device is used), same
+ * status codes.  form: 0 = peeled, 1 = dense.  order_host / pivot_host (nullable, m entries each): step t solves parity
+ * bit pivot[t] from row order[t] (dense: the identity).  P_host (nullable, dense only): m rows of ceil(k / 32) uint32
+ * words, bit j of row i = word j / 32, bit j % 32. */
+int cpb_ldpc_encoder_plan(const int32_t *row_ptr_host, const int32_t *col_idx_host, int m, int n, int force_dense, int *form,
+                          int32_t *order_host, int32_t *pivot_host, uint32_t *P_host);
+/*
+ * Per frame: k message bits from Philox (counter word 0, as cpb_conv_link_tx), encoded as cpb_ldpc_encode does, mapped
+ * bits_per_symbol at a time MSB first (Modem.modulate), + noise_sigma (N(0,1) + j N(0,1)) per symbol (counter word 1, as
+ * cpb_conv_link_tx).  Randomness keyed by (seed, global frame = first_frame + local index).  msg_dev: frames x k uint8;
+ * y_dev: frames x (n / bits_per_symbol) complex64.  CPB_EINVAL when n is not a multiple of bits_per_symbol.
+ */
+int cpb_ldpc_link_tx(const cpbLdpc *h, const cpbModem *modem, int64_t frames, uint64_t seed, int64_t first_frame,
+                     float noise_sigma, uint8_t *msg_dev, float *y_dev, void *stream);
+/* The same over SISO flat fading: symbol s gets its own gain h = (mean_re + j mean_im) + sqrt(nlos / 2) (N(0,1) + j N(0,1))
+ * (counter word 5, as cpb_conv_link_tx_fading) and y = h * point + noise.  h_dev: laid out like y_dev.  With mean = 1,
+ * nlos = 0 the message and y equal cpb_ldpc_link_tx's bit for bit.  CPB_EINVAL also for nlos < 0 or non-finite parameters. */
+int cpb_ldpc_link_tx_fading(const cpbLdpc *h, const cpbModem *modem, int64_t frames, uint64_t seed, int64_t first_frame,
+                            float noise_sigma, float mean_re, float mean_im, float nlos, uint8_t *msg_dev, float *y_dev,
+                            float *h_dev, void *stream);
 
 #ifdef __cplusplus
 }

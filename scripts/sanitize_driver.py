@@ -76,5 +76,20 @@ link = TurboLinkGPU(rsc, RandInterlv(301, 3), 301, frames_per_batch=37, iteratio
 link.link_performance([2.0], send_max=30000, err_min=10 ** 9)
 bpsk_combine(y[:4999], h[:4999])
 bpsk_combine(y[1:], h[:4999])
+# LDPC encoder (peeled and dense forms, a batch that is not a multiple of 32) and the LDPC link over AWGN and fading
+from commpy_b200 import _lib
+from commpy_b200.channelcoding import ldpc_encode_batch
+from commpy_b200.links import LdpcLinkGPU
+Hs = helpers.dvbs2_like_H(n=720, m=360, n8=144, n3=216)
+sparams = {"parity_check_matrix": Hs.tocsc(), "n_vnodes": 720, "n_cnodes": 360}
+smsg = rs.randint(0, 2, (45, 360)).astype(np.uint8)
+ldpc_encode_batch(smsg, sparams)
+_lib.set_option(_lib.OPT_LDPC_ENC_FORCE_DENSE, 1)
+ldpc_encode_batch(smsg, sparams)
+_lib.set_option(_lib.OPT_LDPC_ENC_FORCE_DENSE, 0)
+link = LdpcLinkGPU(sparams, QAMModem(16), 37, n_iters=4, seed=1)
+link.link_performance([8.0], send_max=30000, err_min=10 ** 9)
+link = LdpcLinkGPU(sparams, QAMModem(4), 37, n_iters=4, seed=1, fading_param=(0j, 1))
+link.link_performance([8.0], send_max=30000, err_min=10 ** 9)
 torch.cuda.synchronize()
 print("sanitize driver ok")
