@@ -29,7 +29,7 @@ SYMBOLS = [
     "cpb_modem_create", "cpb_modem_destroy", "cpb_modem_is_separable", "cpb_demod_soft", "cpb_demod_hard",
     "cpb_demod_soft_csi", "cpb_demod_hard_csi",
     "cpb_count_errors", "cpb_conv_link_tx", "cpb_conv_link_tx_punctured", "cpb_conv_link_tx_fading", "cpb_turbo_link_tx",
-    "cpb_turbo_link_tx_fading", "cpb_bpsk_combine",
+    "cpb_turbo_link_tx_fading", "cpb_bpsk_combine", "cpb_turbo_link_tx_modem", "cpb_turbo_link_tx_modem_fading",
     "cpb_ldpc_encode", "cpb_ldpc_encoder_plan", "cpb_ldpc_link_tx", "cpb_ldpc_link_tx_fading",
 ]
 

@@ -25,12 +25,14 @@
 // bytes of syndrome and of parity written and read, m parity bytes written.
 //
 // TX randomness is the conv link's (philox.cuh): message bits from counter word 0, symbol s's noise from word 1 and its
-// flat-fading gain from word 5 (box_muller of the pair (x, y) for even s, (z, w) for odd s of counter s / 2).
+// flat-fading gain from word 5 (box_muller of the pair (x, y) for even s, (z, w) for odd s of counter s / 2), drawn by the
+// shared code-word modulator (codeword_tx.cu).
 #include <algorithm>
 #include <cmath>
 #include <deque>
 #include <vector>
 
+#include "codeword_tx.cuh"
 #include "common.cuh"
 #include "handles.cuh"
 #include "philox.cuh"
@@ -352,62 +354,6 @@ __global__ void __launch_bounds__(256) unpack_parity_kernel(const uint32_t *__re
     }
 }
 
-// ---- device: modulation and channel -------------------------------------------------------------------------------
-struct TxParams {
-    int64_t frames, nsym, npairs, first_frame;
-    int k, m, nb;
-    uint32_t seed_lo, seed_hi;
-    float sigma;
-    float mean_re, mean_im, nlos_std;
-    const float2 *cst;
-    const uint8_t *msg, *par;                            // frames x k, frames x m: code word c = [msg | par]
-    float2 *y, *h;
-};
-
-// h * c; exact at h = 1 + 0j
-__device__ __forceinline__ float2 cmul(float2 h, float2 c)
-{
-    return make_float2(h.x * c.x - h.y * c.y, h.x * c.y + h.y * c.x);
-}
-
-// one thread per (frame, symbol pair): the pair shares a Philox call of the noise (and of the gains)
-template <bool FADING>
-__global__ void __launch_bounds__(256) modulate_kernel(const TxParams p)
-{
-    const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (gid >= p.frames * p.npairs) return;
-    const int64_t fl = gid / p.npairs;
-    const int64_t q = gid - fl * p.npairs;
-    const uint64_t fg = (uint64_t)(p.first_frame + fl);
-    const uint32_t f_lo = (uint32_t)fg, f_hi = (uint32_t)(fg >> 32);
-    const uint4 r = philox4x32_10(make_uint4(f_lo, f_hi, (uint32_t)q, 1u), p.seed_lo, p.seed_hi);
-    const float2 nz[2] = {box_muller(r.x, r.y), box_muller(r.z, r.w)};
-    float2 g[2];
-    if (FADING) {
-        const uint4 rh = philox4x32_10(make_uint4(f_lo, f_hi, (uint32_t)q, 5u), p.seed_lo, p.seed_hi);
-        g[0] = fading_gain(p.nlos_std, p.mean_re, p.mean_im, box_muller(rh.x, rh.y));
-        g[1] = fading_gain(p.nlos_std, p.mean_re, p.mean_im, box_muller(rh.z, rh.w));
-    }
-    const uint8_t *msg = p.msg + fl * p.k;
-    const uint8_t *par = p.par + fl * p.m;
-#pragma unroll
-    for (int u = 0; u < 2; ++u) {
-        const int64_t s = 2 * q + u;
-        if (s >= p.nsym) break;
-        uint32_t idx = 0;
-        for (int b = 0; b < p.nb; ++b) {                 // first code bit of the symbol = MSB (modulation.py:93-96)
-            const int64_t c = s * p.nb + b;
-            idx = (idx << 1) | (uint32_t)(c < p.k ? msg[c] : par[c - p.k]);
-        }
-        float2 c = __ldg(&p.cst[idx]);
-        if (FADING) {
-            p.h[fl * p.nsym + s] = g[u];
-            c = cmul(g[u], c);
-        }
-        p.y[fl * p.nsym + s] = make_float2(fmaf(p.sigma, nz[u].x, c.x), fmaf(p.sigma, nz[u].y, c.y));
-    }
-}
-
 // ---- host: launches -----------------------------------------------------------------------------------------------
 static unsigned blocks(int64_t threads, int per) { return (unsigned)ceil_div(threads, per); }
 
@@ -448,7 +394,7 @@ static int link_tx(const cpbLdpc *h, const cpbModem *md, int64_t frames, uint64_
     if (rc) return rc;
     uint32_t *M = reinterpret_cast<uint32_t *>(ws.ptr), *S = M + (size_t)Wc * p->k, *Pw = S + (size_t)Wc * p->m;
     uint8_t *par = reinterpret_cast<uint8_t *>(Pw + (size_t)Wc * p->m);
-    TxParams tp;
+    cwtx::TxParams tp;
     memset(&tp, 0, sizeof(tp));
     tp.nsym = h->n / nb; tp.npairs = (tp.nsym + 1) / 2;
     tp.k = p->k; tp.m = p->m; tp.nb = nb;
@@ -469,8 +415,7 @@ static int link_tx(const cpbLdpc *h, const cpbModem *md, int64_t frames, uint64_
         tp.msg = msg;
         tp.y = reinterpret_cast<float2 *>(y_dev) + f0 * tp.nsym;
         tp.h = h_dev ? reinterpret_cast<float2 *>(h_dev) + f0 * tp.nsym : nullptr;
-        if (h_dev) modulate_kernel<true><<<blocks(nf * tp.npairs, 256), 256, 0, st>>>(tp);
-        else modulate_kernel<false><<<blocks(nf * tp.npairs, 256), 256, 0, st>>>(tp);
+        cwtx::launch_modulate(tp, h_dev != nullptr, st);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) { ws.release(); return record_cuda_error(e, "ldpc link tx kernels", __FILE__, __LINE__); }
     }

@@ -1,4 +1,4 @@
-// Counter-based random streams of the device TX chains (txlink.cu, turbolink.cu).
+// Counter-based random streams of the device TX chains (txlink.cu, turbolink.cu, ldpclink.cu, codeword_tx.cu).
 //
 // Every random value of global frame f is drawn from Philox4x32-10 with key = seed (lo, hi) and counter
 // (f_lo, f_hi, index, word).  A value depends only on (seed, f, index, word), never on the launch geometry, the batch
@@ -12,8 +12,10 @@
 //     5       conv gains               q       symbols 2q, 2q+1, as the conv noise
 //     5 + j   turbo imaginary noise    q       values 4q .. 4q+3, as the real noise
 //     8 + j   turbo gains              c       values 2c, 2c+1 (one complex gain per box_muller)
+//     0, 1, 5 LDPC link and turbo link over a modem: message bits, noise and gains as the conv link's words 0, 1 and 5
+//             (the noise and gains drawn by the shared code-word modulator, codeword_tx.cu)
 //
-// The two links share words 0 and 5; word 5 is a different stream in each, as no link draws from the other's.
+// The links share words 0 and 5; word 5 is a different stream in the BPSK turbo link, as no link draws from another's.
 #pragma once
 #include <stdint.h>
 

@@ -16,7 +16,9 @@
 * `TurboLinkGPU` is the batched rate-1/3 turbo link over BPSK (`turbo_link_tx` -> cpb_turbo_link_tx, the turbo decoder,
   the error counter).  With `fading_param` it runs over SISO flat fading (`turbo_link_tx_fading` ->
   cpb_turbo_link_tx_fading, one gain per coded bit), and the receiver combines coherently (`bpsk_combine` ->
-  cpb_bpsk_combine, s = Re(conj(h) y)) before the unchanged turbo decoder.
+  cpb_bpsk_combine, s = Re(conj(h) y)) before the unchanged turbo decoder.  With `modem` the code word [sys | par1 | par2]
+  is mapped onto that modem (`turbo_link_tx_modem[_fading]` -> cpb_turbo_link_tx_modem[_fading]), and the receiver hands
+  the demapper's exact LLRs to the same turbo decoder.
 * `LdpcLinkGPU` is the batched LDPC-coded link (`ldpc_link_tx[_fading]` -> cpb_ldpc_link_tx[_fading]: Philox message,
   systematic encoder planned from H, Modem.modulate, AWGN or flat fading), then the demapper, the LDPC decoder and the
   error counter over the message bits.
@@ -30,7 +32,7 @@ import numpy as np
 from . import _lib, parallel
 
 __all__ = ["link_performance", "LinkModel", "AwgnSisoChannel", "ConvLinkGPU", "conv_link_tx", "conv_link_tx_fading",
-           "turbo_link_tx_fading", "bpsk_combine", "idd_decoder", "LdpcLinkGPU", "ldpc_link_tx", "ldpc_link_tx_fading"]
+           "turbo_link_tx_fading", "turbo_link_tx_modem", "turbo_link_tx_modem_fading", "bpsk_combine", "idd_decoder", "LdpcLinkGPU", "ldpc_link_tx", "ldpc_link_tx_fading"]
 
 
 class AwgnSisoChannel:
@@ -603,6 +605,52 @@ def _turbo_link_tx(trellis, interleaver, frames, frame_bits, seed, first_frame, 
     _lib.check(rc, "turbo_link_tx")
     return msg, ys, y1, y2
 
+def turbo_link_tx_modem(trellis, interleaver, modem, frames, frame_bits, seed, first_frame, noise_sigma):
+    """Device-side TX chain of a turbo-coded link over `modem` (cpb_turbo_link_tx_modem): the message of `turbo_link_tx`,
+    the code word c = np.concatenate(turbo_encode(msg, trellis, trellis, interleaver) streams, each cut to frame_bits) =
+    [sys | par1 | par2] -> modem.modulate (MSB first, no channel interleaver) -> + noise_sigma * (N(0,1) + jN(0,1)), the
+    noise stream of `conv_link_tx`.  3 * frame_bits must be a multiple of the modem's bits per symbol.
+
+    Returns (msg uint8 (frames, frame_bits), y complex64 (frames, 3 frame_bits / bits_per_symbol)) as CUDA tensors."""
+    return _turbo_link_tx_modem(trellis, interleaver, modem, frames, frame_bits, seed, first_frame, noise_sigma, None)
+
+
+def turbo_link_tx_modem_fading(trellis, interleaver, modem, frames, frame_bits, seed, first_frame, noise_sigma, fading_param):
+    """`turbo_link_tx_modem` over SISO flat fading (cpb_turbo_link_tx_modem_fading): each symbol c is received as
+    y = h c + noise with its own gain h = fading_param[0] + sqrt(fading_param[1] / 2) * (N(0,1) + jN(0,1)), drawn as
+    `conv_link_tx_fading` draws them.  At fading_param = (1 + 0j, 0) the outputs equal `turbo_link_tx_modem`'s bit for bit.
+
+    Returns (msg uint8 (frames, frame_bits), y complex64 (frames, nsym), h complex64 (frames, nsym)) as CUDA tensors."""
+    return _turbo_link_tx_modem(trellis, interleaver, modem, frames, frame_bits, seed, first_frame, noise_sigma, fading_param)
+
+
+def _turbo_link_tx_modem(trellis, interleaver, modem, frames, frame_bits, seed, first_frame, noise_sigma, fading_param):
+    import ctypes as C
+    from .channelcoding.convcode import _trellis_handle
+    from .channelcoding.turbo import _checked_perm
+    if fading_param is not None:
+        mean, nlos = _fading(fading_param)
+    N, nb = int(frame_bits), int(modem.num_bits_symbol)
+    if (3 * N) % nb:
+        raise ValueError("the code words must fill whole symbols: 3 * %d bits is not a multiple of %d bits per symbol" % (N, nb))
+    torch = _lib.require_cuda()
+    perm = torch.from_numpy(_checked_perm(interleaver, N)).cuda()
+    frames = int(frames)
+    msg = torch.empty((frames, N), dtype=torch.uint8, device="cuda")
+    y = torch.empty((frames, 3 * N // nb), dtype=torch.complex64, device="cuda")
+    lib = _lib.load()
+    head = (_trellis_handle(trellis), modem._handle(), _lib.ptr(perm), C.c_int64(frames), C.c_int64(N),
+            C.c_uint64(int(seed) & ((1 << 64) - 1)), C.c_int64(int(first_frame)), C.c_float(float(noise_sigma)))
+    if fading_param is not None:
+        h = torch.empty_like(y)
+        rc = lib.cpb_turbo_link_tx_modem_fading(*head, C.c_float(mean.real), C.c_float(mean.imag), C.c_float(nlos),
+                                                _lib.ptr(msg), _lib.ptr(y), _lib.ptr(h), _lib.stream_ptr(torch))
+        _lib.check(rc, "turbo_link_tx_modem_fading")
+        return msg, y, h
+    rc = lib.cpb_turbo_link_tx_modem(*head, _lib.ptr(msg), _lib.ptr(y), _lib.stream_ptr(torch))
+    _lib.check(rc, "turbo_link_tx_modem")
+    return msg, y
+
 
 def bpsk_combine(y, h):
     """Coherent BPSK combining (cpb_bpsk_combine): s = Re(conj(h) y) for complex64 CUDA tensors y and h of one shape;
@@ -628,25 +676,46 @@ class TurboLinkGPU:
 
     `fading_param` (a SISOFlatChannel fading_param with a complex mean, e.g. (0j, 1) for Rayleigh): the link runs over i.i.d.
     flat fading, one gain per coded bit (cpb_turbo_link_tx_fading), and the receiver, which knows the gains, combines each
-    value coherently (cpb_bpsk_combine) before the same turbo decoder at the same noise variance; None: AWGN."""
+    value coherently (cpb_bpsk_combine) before the same turbo decoder at the same noise variance; None: AWGN.
 
-    def __init__(self, trellis, interleaver, frame_bits, frames_per_batch=1024, iterations=6, seed=0, fading_param=None):
+    `modem` (a commpy_b200 Modem; 3 * frame_bits must be a multiple of its bits per symbol): the code word [sys | par1 |
+    par2] is mapped onto it (cpb_turbo_link_tx_modem[_fading], one gain per symbol over fading), the receiver demaps with
+    the true complex noise variance N0 (and the gains over fading) into exact LLRs log P(1) / P(0), and the turbo decoder
+    takes the three LLR streams as symbols at noise_variance = 2, where its channel term 2 r / nv is the LLR itself.
+    None: BPSK, one real value per coded bit, every path as without the argument."""
+
+    def __init__(self, trellis, interleaver, frame_bits, frames_per_batch=1024, iterations=6, seed=0, fading_param=None,
+                 modem=None):
         self.fading_param = fading_param
         if fading_param is not None:
             _fading(fading_param)
-        self.trellis, self.interleaver = trellis, interleaver
+        if modem is not None and (3 * int(frame_bits)) % int(modem.num_bits_symbol):
+            raise ValueError("the code words must fill whole symbols: 3 * %d bits is not a multiple of %d bits per symbol"
+                             % (int(frame_bits), int(modem.num_bits_symbol)))
+        self.trellis, self.interleaver, self.modem = trellis, interleaver, modem
         self.frame_bits, self.frames, self.iterations, self.seed = int(frame_bits), int(frames_per_batch), int(iterations), int(seed)
 
     def noise_variance(self, ebn0_db):
         """sigma^2 per real component at Eb/N0 (dB) for rate 1/3 and Es = 1; over fading E|h|^2 = 1 for every valid
-        fading_param, so Eb/N0 is the mean Eb/N0."""
+        fading_param, so Eb/N0 is the mean Eb/N0.  With a modem: sigma^2 = Es / (2 R nb Eb/N0), nb bits per symbol of
+        energy Es (the reference's SISOFlatChannel.set_SNR_dB(EbN0 + 10 log10 nb, 1/3, Es), channels.py:74)."""
+        if self.modem is not None:
+            nb = int(self.modem.num_bits_symbol)
+            return float(self.modem.Es) / (2.0 * (1.0 / 3.0) * nb * 10 ** (ebn0_db / 10.0))
         return 1.0 / (2.0 * (1.0 / 3.0) * 10 ** (ebn0_db / 10.0))
 
     def make_batch(self, ebn0_db, batch_index):
-        """(msg, sys, par1, par2, sigma^2) over AWGN; (msg, y, h, sigma^2) over fading (y, h: (3, frames, frame_bits))."""
+        """(msg, sys, par1, par2, sigma^2) over AWGN; (msg, y, h, sigma^2) over fading (y, h: (3, frames, frame_bits)).
+        With a modem: (msg, y, N0) over AWGN and (msg, y, h, N0) over fading, y and h (frames, 3 frame_bits / nb) and
+        N0 = 2 sigma^2 the complex noise variance."""
         rank, world, _ = parallel.world()
         first = parallel.batch_first_frame(batch_index, self.frames, rank, max(world, 1))
         s2 = self.noise_variance(ebn0_db)
+        if self.modem is not None:
+            args = (self.trellis, self.interleaver, self.modem, self.frames, self.frame_bits, self.seed, first, math.sqrt(s2))
+            if self.fading_param is not None:
+                return turbo_link_tx_modem_fading(*args, self.fading_param) + (2.0 * s2,)
+            return turbo_link_tx_modem(*args) + (2.0 * s2,)
         if self.fading_param is not None:
             return turbo_link_tx_fading(self.trellis, self.interleaver, self.frames, self.frame_bits, self.seed, first,
                                         math.sqrt(s2), self.fading_param) + (s2,)
@@ -654,9 +723,15 @@ class TurboLinkGPU:
 
     def decode_count(self, msg, *args):
         """decode_count(*make_batch(...), counters, torch): decode(msg, sys, par1, par2, s2, counters, torch) over AWGN,
-        (msg, y, h, s2, counters, torch) over fading -- y and h are combined first.  Adds the errors to `counters`."""
+        (msg, y, h, s2, counters, torch) over fading -- y and h are combined first.  Adds the errors to `counters`.
+        With a modem: (msg, y, N0, counters, torch) or (msg, y, h, N0, counters, torch)."""
         from .channelcoding import turbo_decode_batch
         *rx, s2, counters, torch = args
+        if self.modem is not None:
+            ys, y1, y2 = self.llr_streams(*rx, s2)
+            dec = turbo_decode_batch(ys, y1, y2, self.trellis, 2.0, self.iterations, self.interleaver)
+            _count_errors(dec, msg, counters, torch)
+            return dec
         if self.fading_param is not None:
             y, h = rx
             ys, y1, y2 = bpsk_combine(y, h)
@@ -665,6 +740,14 @@ class TurboLinkGPU:
         dec = turbo_decode_batch(ys, y1, y2, self.trellis, s2, self.iterations, self.interleaver)
         _count_errors(dec, msg, counters, torch)
         return dec
+
+    def llr_streams(self, y, *rest):
+        """llr_streams(y, N0) or (y, h, N0) of a modem link: the demapper's exact LLRs log P(1) / P(0) of the (frames, 3N)
+        code bits (no clamp), split into three contiguous (frames, N) float32 streams sys, par1, par2."""
+        *h, N0 = rest
+        llr = self.modem.demodulate_batch(y, "soft", N0, h[0] if h else None).view(y.shape[0], 3 * self.frame_bits)
+        N = self.frame_bits
+        return tuple(llr[:, j * N:(j + 1) * N].contiguous() for j in range(3))
 
     def link_performance(self, EbN0s, send_max, err_min):
         """BER per Eb/N0 (dB): a point ends when the global counters reach `err_min` bit errors or `send_max` bits."""

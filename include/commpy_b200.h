@@ -266,6 +266,21 @@ int cpb_turbo_link_tx_fading(const cpbTrellis *t, const int32_t *perm_dev, int64
  * cpb_map_decode / cpb_turbo_decode take s with noise_variance = sigma^2 and decode exactly.  s = Re(y) where h = 1 + 0j,
  * 0 where h = 0. */
 int cpb_bpsk_combine(const float *y_dev, const float *h_dev, int64_t n, float *s_dev, void *stream);
+/* The same turbo code over a modem (bit-interleaved coded modulation without a channel interleaver): per frame the code word
+ * c = [sys | par1 | par2] (3N bits, the streams of cpb_turbo_link_tx, sys = msg) is mapped bits_per_symbol at a time MSB
+ * first (Modem.modulate) and disturbed by noise_sigma (N(0,1) + j N(0,1)) per symbol.  The message is cpb_turbo_link_tx's
+ * (counter word 0) bit for bit; the noise is Philox counter word 1, as in cpb_conv_link_tx.  msg_dev: frames x N uint8;
+ * y_dev: frames x (3N / bits_per_symbol) complex64.  CPB_EINVAL for null pointers, N < 1, first_frame < 0 and
+ * 3N % bits_per_symbol != 0; CPB_EUNSUPPORTED for a trellis cpb_turbo_link_tx refuses. */
+int cpb_turbo_link_tx_modem(const cpbTrellis *t, const cpbModem *modem, const int32_t *perm_dev, int64_t frames, int64_t N,
+                            uint64_t seed, int64_t first_frame, float noise_sigma, uint8_t *msg_dev, float *y_dev, void *stream);
+/* The same over SISO flat fading: symbol s gets its own gain h = (mean_re + j mean_im) + sqrt(nlos / 2) (N(0,1) + j N(0,1))
+ * (counter word 5, as cpb_conv_link_tx_fading) and y = h * point + noise.  h_dev: laid out like y_dev.  With mean = 1,
+ * nlos = 0 the message and y equal cpb_turbo_link_tx_modem's bit for bit.  CPB_EINVAL also for nlos < 0 or non-finite
+ * parameters. */
+int cpb_turbo_link_tx_modem_fading(const cpbTrellis *t, const cpbModem *modem, const int32_t *perm_dev, int64_t frames,
+                                   int64_t N, uint64_t seed, int64_t first_frame, float noise_sigma, float mean_re, float mean_im,
+                                   float nlos, uint8_t *msg_dev, float *y_dev, float *h_dev, void *stream);
 
 /* ---- LDPC systematic encoding and the transmit side of an LDPC-coded link: commpy/channelcoding/ldpc.py:302-354
  * (triang_ldpc_systematic_encode) + Modem.modulate + AWGN / SISO flat fading (channels.py:176-221) ---- */

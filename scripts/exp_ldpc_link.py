@@ -39,7 +39,8 @@ def timed(fn, calls, warmup=2):
 
 
 def kernel_times(fn, calls=5):
-    """mean device time (s) per launch of each ldpclink kernel over `calls` calls of fn(), from torch.profiler"""
+    """mean device time (s) per launch of each ldpclink kernel, and of the shared code-word modulator (cwtx::), over `calls`
+    calls of fn(), from torch.profiler"""
     from torch.profiler import ProfilerActivity, profile
     fn()
     torch.cuda.synchronize()
@@ -49,7 +50,7 @@ def kernel_times(fn, calls=5):
         torch.cuda.synchronize()
     out = {}
     for e in prof.key_averages():
-        if "ldpclink::" in e.key and e.count:
+        if ("ldpclink::" in e.key or "cwtx::" in e.key) and e.count:
             t = getattr(e, "device_time_total", None)
             t = e.cuda_time_total if t is None else t
             out[e.key.split("(")[0]] = t * 1e-6 / e.count

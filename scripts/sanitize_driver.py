@@ -91,5 +91,14 @@ link = LdpcLinkGPU(sparams, QAMModem(16), 37, n_iters=4, seed=1)
 link.link_performance([8.0], send_max=30000, err_min=10 ** 9)
 link = LdpcLinkGPU(sparams, QAMModem(4), 37, n_iters=4, seed=1, fading_param=(0j, 1))
 link.link_performance([8.0], send_max=30000, err_min=10 ** 9)
+# turbo link over a modem: parity kernel on its byte path (N = 301) and 16-byte path (N = 512), both modem TX entry points
+from commpy_b200.links import turbo_link_tx_modem, turbo_link_tx_modem_fading
+link = TurboLinkGPU(rsc, RandInterlv(301, 3), 301, frames_per_batch=37, iterations=2, seed=1, modem=PSKModem(8))
+link.link_performance([4.0], send_max=30000, err_min=10 ** 9)
+link = TurboLinkGPU(rsc, RandInterlv(512, 3), 512, frames_per_batch=37, iterations=2, seed=1, fading_param=(0j, 1),
+                    modem=QAMModem(16))
+link.link_performance([6.0], send_max=30000, err_min=10 ** 9)
+turbo_link_tx_modem(rsc, RandInterlv(512, 2), QAMModem(256), 33, 512, 3, 5, 0.5)
+turbo_link_tx_modem_fading(rsc, RandInterlv(301, 2), PSKModem(8), 33, 301, 3, 5, 0.5, (0.6 + 0j, 0.64))
 torch.cuda.synchronize()
 print("sanitize driver ok")
